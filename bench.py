@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- WCSPH step throughput on B200 (contract: see the task statement / DESIGN.md section 6).
+"""bench.py -- WCSPH step throughput on H100 (DESIGN.md section 6).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--scene NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--scene NAME] [--dump-outputs DIR]
 
 One "step" is one full ``SPHBase.step()`` (neighbour build + density + forces + integration +
 walls, sph_base.py:263-271 of the reference) over the named scene.  N = 1 runs BASELINE config 2
@@ -13,6 +13,10 @@ flushed between timed steps; ``steady`` = back-to-back steps (state L2-resident,
 simulation actually runs); ``e2e`` = the same through the public Python surface with pinned HOST
 buffers (H2D of x, v and D2H of x, v every step); ``roofline`` for the force kernel;
 ``cpu_baseline`` = the CPU oracle port on this box's cores (bounded sample).
+
+--dump-outputs DIR (single GPU) writes the state after the last step of the first timed window (x, v,
+density, pressure and the rest position x_0, float32, rows ordered by (object_id, x_0)) as DIR/<name>.npy,
+so that two builds can be compared output for output on the same seeded scene.
 """
 from __future__ import annotations
 
@@ -33,14 +37,14 @@ def pin_openmp_for_the_cpu_arm():
     """The CPU arm pins its OpenMP threads (must happen before libgomp initialises, i.e. before torch or the oracle are
     imported); the thread COUNT is chosen in best_thread_count.  NEVER in a multi-rank run: with OMP_NUM_THREADS=1
     (torchrun's default) the binding pins the main thread of EVERY rank to the first place -- all ranks time-slice one
-    core and the asynchronous launches of a sharded step crawl (1.44 instead of 0.45 ms per step at 4 GPUs)."""
+    core and the asynchronous launches of a sharded step crawl."""
     os.environ.setdefault("OMP_PROC_BIND", "close")
     os.environ.setdefault("OMP_PLACES", "cores")
 
 METRIC = "M particle-updates/sec (SPH steps/sec x particles)"
 UNIT = "M particle-updates/s"
 FORCE_BYTES_PER_PARTICLE = 52  # SURVEY.md section 8d: algorithmic bytes of the force pass
-HBM_FALLBACK_GBS = 6650.0      # /opt/skills/guides/B200_PROFILING.md
+HBM_FALLBACK_GBS = 3350.0      # H100 SXM data sheet (HBM3)
 
 
 def scene_for(n_gpus, name=None):
@@ -51,7 +55,7 @@ def scene_for(n_gpus, name=None):
 
 
 def workload_config(name, sc, particles, fluid_particles):
-    """The `config` object -- identical (keys AND values) in the B200 arm and in the --impl reference arm."""
+    """The `config` object -- identical (keys AND values) in the GPU arm and in the --impl reference arm."""
     import numpy as np
     c = sc["Configuration"]
     ds = np.array(c["domainEnd"], dtype=np.float64) - np.array(c["domainStart"], dtype=np.float64)
@@ -59,9 +63,9 @@ def workload_config(name, sc, particles, fluid_particles):
     return {"workload": name, "particles": int(particles), "fluid_particles": int(fluid_particles), "grid_cells": cells,
             "solver": "WCSPH" if c["simulationMethod"] == 0 else "DFSPH", "dt": c["timeStepSize"],
             "state": "the scene after `warmup` steps from its initial lattice",
-            "l2": "B200 arm: L2 flushed between timed steps at N = 1 (256 MiB write; 'steady' is un-flushed), per-rank "
+            "l2": "GPU arm: L2 flushed between timed steps at N = 1 (256 MiB write; 'steady' is un-flushed), per-rank "
                   "working set > L2 at N > 1; reference arm: CPU caches not flushed",
-            "parallelism": "B200 arm: N = 1 single GPU, N > 1 x-slabs with one halo exchange per step; reference arm: "
+            "parallelism": "GPU arm: N = 1 single GPU, N > 1 x-slabs with one halo exchange per step; reference arm: "
                            "OpenMP over the host cores"}
 
 
@@ -71,11 +75,11 @@ def measured_hbm_peak():
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+        return HBM_FALLBACK_GBS, "fallback (H100 SXM data sheet)"
 
 
 def ncu_dram_traffic(workload, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one kernel, per launch, from this round's committed
+    """dram__bytes_read.sum + dram__bytes_write.sum of one kernel, per launch, from a committed
     ncu --set full capture of the same workload (profiles/dram_traffic.json names the capture), else None."""
     try:
         with open(os.path.join(ROOT, "profiles", "dram_traffic.json")) as fh:
@@ -93,7 +97,7 @@ KERNEL_NAME = {"density": "density pass (k_density_*: scan + neighbour lists + E
                "force": "k_force_packed<4,128,true> (cohesion + viscosity + pressure gradient + integration + walls)"}
 
 
-def roofline_entry(kind, workload, n, launch_ms, total_ms, peak, work, sm_mhz):
+def roofline_entry(kind, workload, n, launch_ms, total_ms, peak, work, sm_mhz, sms):
     ach = ALGO_BYTES[kind] * n / (launch_ms * 1e-3) / 1e9 if launch_ms > 0 else 0.0
     e = {"kernel": KERNEL_NAME[kind], "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
          "frac": ach / peak, "traffic": ncu_dram_traffic(workload, kind),
@@ -102,10 +106,10 @@ def roofline_entry(kind, workload, n, launch_ms, total_ms, peak, work, sm_mhz):
     if work and "candidate_tests_per_pass" in work and sm_mhz:
         ops = (work["candidate_tests_per_pass"] * LANE_OPS_PER_TEST + work["accepted_pairs_per_pass"] * LANE_OPS_PER_DENSITY_HIT
                if kind == "density" else work["accepted_pairs_per_pass"] * LANE_OPS_PER_FORCE_PAIR)
-        lane_peak = 148 * 128 * sm_mhz * 1e6
+        lane_peak = sms * 128 * sm_mhz * 1e6
         e["compute_side"] = {"fp32_lane_ops_per_launch": int(ops), "achieved_lane_ops_per_s": ops / (launch_ms * 1e-3),
                              "peak_lane_ops_per_s": lane_peak, "frac": ops / (launch_ms * 1e-3) / lane_peak,
-                             "formula": "density: tests x 7 + pairs x 30; force: pairs x 54; peak = 148 SMs x 128 lanes x SM clock"}
+                             "formula": f"density: tests x 7 + pairs x 30; force: pairs x 54; peak = {sms} SMs x 128 lanes x SM clock"}
     return e
 
 
@@ -114,16 +118,16 @@ class ClockSampler:
     """SM clock and throttle reasons sampled WHILE the timed region runs.
 
     In-process NVML (pynvml) from a thread, one cheap query pair every 10 ms: `nvidia-smi -lms 20` as a child process
-    stalled the sampled GPU for milliseconds per poll -- invisible in a 4 s region, but +46 % on the 10 ms timed
-    region of a sharded run (profiles/r02_shard_timing.txt).  Falls back to `nvidia-smi -lms 100` without pynvml."""
+    stalled the sampled GPU for milliseconds per poll -- invisible in a long region, but large on the short timed
+    region of a sharded run.  Falls back to `nvidia-smi -lms 100` without pynvml."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
     BITS = {"hw_slowdown": 0x8, "hw_thermal_slowdown": 0x40, "sw_thermal_slowdown": 0x20, "sw_power_cap": 0x4}
 
     def __init__(self, index=0):
-        """Construct EARLY (before the warm-up): nvmlInit enumerates the devices and stalls them for ~100 ms -- it must
-        not fall into the timed region (it did: 3.3 instead of 0.78 ms/step over a 16 ms region)."""
+        """Construct EARLY (before the warm-up): nvmlInit enumerates the devices and stalls them -- it must
+        not fall into the timed region (it would dominate a timed region of a few ms)."""
         self.rows, self.sm, self.reasons = [], [], set()
         self.proc = self.thread = self.nvml = None
         self.index = index
@@ -209,10 +213,8 @@ class ClockSampler:
 def best_thread_count(o, reps=3):
     """Give the CPU arm its best shot: the pair loops are memory-latency bound and SMT siblings can hurt, so
     time `reps` steps (after one step) at cpu_count / 8, / 4, / 2 and cpu_count threads (plus the cgroup CPU quota when the
-    box has one -- on this pool 128 threads run at 0.7 steps/s against 14 at 16-32, the signature of a quota well
-    below the visible thread count, see profiles/r02_cpu_arm_binding.txt) and keep the fastest.  Returns
-    (best, {threads: steps/s}) -- round 1 timed ONE step per candidate and picked 32 threads on one box and 64 on
-    another for the same scene (3.5x swing in the reference arm)."""
+    box has one: a host can expose many more threads than it schedules) and keep the fastest.  Returns
+    (best, {threads: steps/s}) -- timing ONE step per candidate picked different counts on equal hosts."""
     from oracle.sph_oracle import set_threads
     total = os.cpu_count() or 1
     table = {}
@@ -221,8 +223,8 @@ def best_thread_count(o, reps=3):
     if quota:
         cand.add(max(1, min(total, int(quota))))
     # ascending, and stop at the first count whose FIRST step is already twice as slow as the best so far: past the
-    # cores the box really schedules, more threads only get worse (128 threads: 0.7 steps/s against 14 at 16-32 on
-    # this pool), and on the 16 M-particle scene of the 8-GPU reference arm one such step costs a minute
+    # cores the box really schedules, more threads only get worse, and on the 16 M-particle scene of the 8-GPU
+    # reference arm one such step costs a minute
     best_step = None
     for n in sorted(cand):
         set_threads(n)
@@ -360,7 +362,7 @@ def run_single(args):
     eng = ps._engine
     n = ps.particle_max_num
     K, W = args.steps, args.warmup
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     solver.step(W)
     eng.check_status()
@@ -384,6 +386,8 @@ def run_single(args):
         torch.cuda.synchronize()
         launches = eng.launch_count() - launches0
         cold_ms = sum(a.elapsed_time(b) for a, b in ev)
+        if attempt == 0 and args.dump_outputs:  # the first window: W + 3 + K steps whether or not it is re-measured
+            outputs = snapshot_outputs(ps)
         # ---- steady state: K back-to-back steps (state stays in L2, as in a real run) ----
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         torch.cuda.synchronize()
@@ -459,7 +463,8 @@ def run_single(args):
     val = K / (cold_ms * 1e-3)
     total_ms = stages.get("total", 0.0)
     work = compute if compute and "error" not in compute else None
-    kernels = [roofline_entry(kind, name, n, stages.get(kind, 0.0), total_ms, peak, work, clocks.get("sm_mhz"))
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    kernels = [roofline_entry(kind, name, n, stages.get(kind, 0.0), total_ms, peak, work, clocks.get("sm_mhz"), sms)
                for kind in ("density", "force") if stages.get(kind, 0.0) > 0]
     kernels.sort(key=lambda e: -e["avg_launch_ms"])
     roof = dict(kernels[0]) if kernels else {"bound": "hbm", "achieved": 0.0, "peak": peak, "unit": "GB/s", "frac": 0.0,
@@ -494,8 +499,36 @@ def run_single(args):
         "extra_configs": extra,
         "cpu_baseline": cpu,
     }
+    if args.dump_outputs:
+        write_outputs(args.dump_outputs, outputs)
     print(json.dumps(line))
     return 0
+
+
+DUMP_FIELDS = ("x", "v", "density", "pressure", "x_0")
+DUMP_MAX_BYTES = 64_000_000 - 64 * 1024  # 64 MB in all, with room for the .npy headers
+
+
+def snapshot_outputs(ps):
+    """The per-particle state a caller of solver.step() reads, as float32, rows ordered by (object_id, x_0): the
+    engine's particle order is a detail of the neighbour sort, the rest position identifies a particle.  Above
+    DUMP_MAX_BYTES a fixed seeded sample of the rows is kept."""
+    import numpy as np
+    x0, oid = ps.x_0.to_numpy(), ps.object_id.to_numpy()
+    rows = np.lexsort((x0[:, 2], x0[:, 1], x0[:, 0], oid))
+    out = {k: getattr(ps, k).to_numpy()[rows].astype(np.float32) for k in DUMP_FIELDS}
+    row_bytes = sum(a[0].nbytes for a in out.values())
+    if row_bytes * len(rows) > DUMP_MAX_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(len(rows), DUMP_MAX_BYTES // row_bytes, replace=False))
+        out = {k: a[keep] for k, a in out.items()}
+    return out
+
+
+def write_outputs(out_dir, arrays):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def extra_leg(name, steps, warmup):
@@ -540,7 +573,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=50)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--scene", default=None)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the state after the last timed step as DIR/<name>.npy (single GPU)")
     args = ap.parse_args()
+    multi = args.gpus > 1 or int(os.environ.get("WORLD_SIZE", "1")) > 1
+    if args.dump_outputs and (multi or args.impl != "b200"):
+        ap.error("--dump-outputs is implemented for the single-GPU run of the CUDA engine")
     if args.warmup < 3:
         args.warmup = 3
     if args.impl == "reference":

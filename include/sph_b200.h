@@ -1,5 +1,5 @@
 /*
- * sph_b200.h -- C ABI of libsph_b200.so, the sm_100a WCSPH step engine.
+ * sph_b200.h -- C ABI of libsph_b200.so, the sm_90a (H100) WCSPH step engine.
  *
  * The reference (erizmr/SPH_Taichi @ 4a701fd) is pure Python + Taichi and has NO FFI of its
  * own: the drop-in boundary is the Python class surface ParticleSystem / SPHBase /
@@ -177,9 +177,8 @@ int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double et
  * build, moving boundary volumes, compute_densities, compute_DFSPH_factor, divergence_solve (if enabled),
  * compute_non_pressure_forces, predict_velocity, pressure_solve, advect, solve_rigid_body, enforce_boundary_3D(fluid)
  * -- every kernel launched from this one call, the two Jacobi loops run as in sph_dfsph_solve.  A DFSPH step is
- * ~50 launches; this keeps the host out of the way (dragon_bath_dfsph: 1.94 ms per step, 2.00 driven op by op with
- * sph_dfsph_solve, 2.22 with host loops; the step is bound by its ~12 Jacobi sweeps of ~105 us).  The caller fills the
- * constants exactly as the reference's host code computes them. */
+ * ~50 launches; issuing them all from C++ keeps the Python host loop out of the way (the step is then bound by its
+ * Jacobi sweeps).  The caller fills the constants exactly as the reference's host code computes them. */
 typedef struct SphDfsphStep {
     int32_t enable_divergence_solver;   /* DFSPH.py:12 */
     int32_t max_iterations_v, max_iterations; /* m_max_iterations_v, m_max_iterations */

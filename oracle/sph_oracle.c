@@ -6,7 +6,7 @@
  * algorithm line by line and is pinned three ways:
  *   (1) tests/test_golden_reference.py -- golden vectors written by the reference's OWN source
  *       files (particle_system.py, sph_base.py, WCSPH.py, DFSPH.py, imported unmodified from
- *       /root/reference) executed under a pure-Python stand-in for the Taichi runtime
+ *       a reference checkout) executed under a pure-Python stand-in for the Taichi runtime
  *       (tests/golden/ti_shim/: serial loops, IEEE float32; tests/golden/make_reference_golden.py).
  *       This pins the algorithm as written in the reference; it is NOT a run of Taichi's
  *       code generator (fast-math, atomics order), which remains unavailable offline;

@@ -25,7 +25,7 @@ def write_ply_ascii(path, pos):
 
 
 if __name__ == "__main__":
-    parser = argparse.ArgumentParser(description="SPH (B200 engine)")
+    parser = argparse.ArgumentParser(description="SPH (CUDA engine)")
     parser.add_argument("--scene_file", default="", help="scene file (JSON, the reference's schema)")
     parser.add_argument("--scene", default="", help="built-in scene name instead of a file, e.g. dragon_bath "
                                                     "(python -m sph_taichi_b200.scene DIR writes them as JSON)")

@@ -8,8 +8,7 @@ against the oracle):
 
 * ``device_side_loops = True`` (default): ``step()`` is ONE library call (``sph_dfsph_step``) that launches the
   ~50 kernels of a step back to back and runs the two Jacobi loops with the loop condition evaluated on the device
-  after every sweep -- one host wait per batch of sweeps, the first batch sized by the previous step's count
-  (dragon_bath_dfsph: 1.94 ms per step against 2.22 with the host loops).
+  after every sweep -- one host wait per batch of sweeps, the first batch sized by the previous step's count.
   ``divergence_solve()`` / ``pressure_solve()`` called on their own use ``sph_dfsph_solve`` for the loop.
 * ``False`` (or ``SPH_DFSPH_HOST_LOOPS=1``): the reference's structure -- every method below is one launch and the
   loops run on the host (``divergence_solver_iteration`` / ``pressure_solve_iteration``: one density-error read-back

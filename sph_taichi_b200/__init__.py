@@ -1,4 +1,4 @@
-"""sph_taichi_b200: a Blackwell-native (sm_100a) WCSPH step engine behind the
+"""sph_taichi_b200: a Hopper-native (sm_90a) WCSPH step engine behind the
 ParticleSystem / SPHBase.step() surface of erizmr/SPH_Taichi."""
 from .config_builder import SimConfig  # noqa: F401
 

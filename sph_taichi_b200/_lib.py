@@ -14,7 +14,7 @@ _ROOT = os.path.dirname(_PKG)
 LIB_PATH = os.environ.get("SPH_B200_LIB") or os.path.join(_PKG, "libsph_b200.so")  # override: experiments only
 CSRC = os.path.join(_PKG, "csrc")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC", "-ldl"]
 
 # every symbol include/sph_b200.h declares (tests check the .so exports all of them)
@@ -36,7 +36,7 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/sph_b200.cu for sm_100a into the in-tree shared library."""
+    """Compile csrc/sph_b200.cu for sm_90a (H100) into the in-tree shared library."""
     srcs = sources()
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(s) for s in srcs):
         return LIB_PATH

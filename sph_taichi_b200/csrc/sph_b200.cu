@@ -117,6 +117,7 @@ struct SphCtx {
     DevArrays S;
     Layout L;
     int device = 0;
+    int sms = 1;  // multiprocessors of `device` (sizes the grid-stride grids of sharded steps)
     int64_t n_max = 0, n_solid_cap = 0;
     int body_cap = 0;
     char *ws = nullptr;
@@ -148,9 +149,9 @@ struct SphCtx {
     cudaGraphExec_t graph_shard[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [parity][wide exchange]
     int64_t graph_shard_kernels[2][2] = {{0, 0}, {0, 0}};
     int32_t narrow_cap = 0;      // records per side of the usual (sgw + 1 layers) exchange; halo_cap = sgw + 2 layers
-    // hide the exchange behind the interior densities too (boundary densities first): pays off when a rank talks to
-    // two neighbours and the exchange outlasts the interior force pass (8 ranks: 0.38 vs 0.2 ms); with one neighbour
-    // or short exchanges the second density launch costs more than it hides (4 ranks: 0.457 vs 0.444 ms per step)
+    // hide the exchange behind the interior densities too (boundary densities first): meant for a rank that talks to
+    // two neighbours, whose exchange can outlast the interior force pass; with one neighbour or short exchanges the
+    // second density launch can cost more than it hides (not measured on H100s)
     bool split_density = false;
     int64_t shard_sequences = 0;  // sequences run so far (begin = 0): sequence q feeds the plan kernel of q + 1
 };
@@ -222,17 +223,15 @@ inline RigidBodyDev *dev_bodies(SphCtx *c) { return reinterpret_cast<RigidBodyDe
 inline int blocks_for(int64_t n, int t) { return (int)((n + t - 1) / t); }
 // Sharded steps: n is the capacity and the real counts are device state, so the LIGHT step kernels (histogram,
 // bucket, rank + move) run grid-stride loops over the compact input numbering on a grid of `per_sm` resident blocks
-// per SM instead of one thread per capacity slot (sort chain 0.121 -> 0.106 ms at 2 M particles per rank); the pair
-// kernels keep one block per tile.
-constexpr int kSMs = 148;
+// per SM instead of one thread per capacity slot; the pair kernels keep one block per tile.
 inline int step_grid(const SphCtx *c, int64_t n, int t, int per_sm) {
     const int full = blocks_for(n, t);
-    return c->P.slab_on ? std::min(full, kSMs * per_sm) : full;
+    return c->P.slab_on ? std::min(full, c->sms * per_sm) : full;
 }
 
 // Launch with programmatic stream serialisation (the kernels of the step chain start with pdl_wait()): the next
-// kernel's blocks are scheduled while the previous grid drains, which removes most of the ~1.5 us gap per graph
-// node.  SPH_PDL=0 switches it off (A/B).
+// kernel's blocks are scheduled while the previous grid drains, which hides most of the launch gap between graph
+// nodes.  SPH_PDL=0 switches it off (A/B).
 #ifdef SPH_EMU
 #define PDL_LAUNCH(kern, grid, block, st, ...) kern<<<grid, block, 0, st>>>(__VA_ARGS__)
 #else
@@ -413,6 +412,8 @@ int sph_create(const SphParams *params, int64_t n_max, int64_t n_solid, int32_t 
     if (!c) return fail(nullptr, SPH_E_CAPACITY, "out of host memory");
     c->hp = *params;
     c->device = device;
+    e = cudaDeviceGetAttribute(&c->sms, cudaDevAttrMultiProcessorCount, device);
+    if (e != cudaSuccess) { delete c; return fail(nullptr, SPH_E_CUDA, cudaGetErrorString(e)); }
     c->n_max = n_max;
     c->n_solid_cap = n_solid;
     c->body_cap = n_bodies;
@@ -970,8 +971,8 @@ int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // Un-graphed launches are the DEFAULT here: nothing in a sharded step waits for the host any more, so the launches
     // run ahead of the device, and a graph replay -- whose two branches (exchange || interior forces) must both finish
-    // before the next replay may start -- measured 9-12 % SLOWER (0.779 vs 0.712 ms per step at 2 x 2 M particles,
-    // 0.51 vs 0.45 at 4 x 1 M; profiles/r02_shard_timing.txt).  SPH_SHARD_GRAPH=1 replays the captured graph instead
+    // before the next replay may start -- holds back the next step's first kernels, which un-graphed launches queue
+    // behind the interior pass (not measured on H100s).  SPH_SHARD_GRAPH=1 replays the captured graph instead
     // (one graph per ping-pong parity and exchange width; pays off for small per-rank problems).
     static const bool eager = !(std::getenv("SPH_SHARD_GRAPH") && std::atoi(std::getenv("SPH_SHARD_GRAPH")) != 0);
     for (int s = 0; s < nsteps; ++s) {

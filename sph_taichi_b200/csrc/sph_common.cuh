@@ -1,4 +1,4 @@
-// sph_common.cuh -- shared device-side types and math for libsph_b200 (sm_100a).
+// sph_common.cuh -- shared device-side types and math for libsph_b200 (sm_90a).
 //
 // Data layout in HBM (all arrays sorted by flattened cell id, z fastest, like the reference's
 // counting sort; particle_system.py:292-294,322-369).  Everything a pair kernel gathers per
@@ -61,7 +61,7 @@ struct DevParams {
     int32_t opaque_zero;  // always 0; lets a kernel state a scheduling dependency ptxas cannot fold away
     // nibble p = the (dx, dy) column c = (dx + 1) * 3 + (dy + 1) the density pass visits p-th.  The list order is
     // free (only the summation order of the pair passes depends on it); centre column first makes the lanes of
-    // a warp gather the SAME records at the same time in the force pass (profiles/r02_column_order.txt)
+    // a warp gather the SAME records at the same time in the force pass
     unsigned long long col_order;
 };
 

@@ -1,4 +1,4 @@
-// sph_kernels.cuh -- device kernels of libsph_b200 (sm_100a).  See sph_common.cuh for layout.
+// sph_kernels.cuh -- device kernels of libsph_b200 (sm_90a).  See sph_common.cuh for layout.
 #pragma once
 #include "sph_common.cuh"
 
@@ -792,7 +792,7 @@ __global__ void __launch_bounds__(RIGID_THREADS) k_rigid(DevParams P, DevArrays 
 }
 
 // =====================================================================================
-// Production pair kernels.  History and measurements: DESIGN.md section 3.1, profiles/.
+// Production pair kernels.  History: DESIGN.md section 3.1.
 //
 //  * The density pass scans the 27-cell candidates once per step and appends the accepted pairs
 //    to a per-particle neighbour list (reference visiting order); the force pass is a dense loop
@@ -880,7 +880,7 @@ __device__ __forceinline__ uint32_t scan_chunk(const DevParams &P, const float4 
 // INLINE_W: the density contribution of a hit is taken from the staged window while flushing the
 // bitmask; otherwise a second dense loop re-gathers the neighbours from global memory.
 #ifndef DENS_MIN_BLOCKS
-#define DENS_MIN_BLOCKS 9  // 56 registers: measured best (profiles/, DESIGN.md section 3.1)
+#define DENS_MIN_BLOCKS 8  // H100 sweep of 7-10 blocks/SM: 8 is fastest on dragon_bath and armadillo (DESIGN.md 3.1)
 #endif
 // FASTW (with INLINE_W): the branch-free spline_w_norm() with the 2k factor applied once per particle;
 // DFSPH keeps the reference's piecewise form (its solver loops count iterations against the oracle).
@@ -902,8 +902,8 @@ __global__ void __launch_bounds__(DENS_WARPS * 32, DENS_MIN_BLOCKS) k_density_tm
     auto tile = [&](const int i) {
     bool live = i < P.n;
     if (P.slab_on) {
-        // sharded steps: the grid covers the capacity (the hardware block scheduler balances better than a persistent
-        // tile loop: 0.385 vs 0.49 ms at 2 M particles per rank, profiles/r02_shard_timing.txt); only owned particles
+        // sharded steps: the grid covers the capacity (the hardware block scheduler balanced better than a persistent
+        // tile loop when both were tried); only owned particles
         // + the first ghost layer per side -- one index range of the device-resident step state -- need a density
         const int32_t *sd = S.sd;
         live = i >= sd[SD_DENS0] && i < sd[SD_DENS1];
@@ -1167,7 +1167,7 @@ __device__ __forceinline__ void force_pair_packed(const DevParams &P, const DevA
 // epilogue integrate the particle and clamp it to the walls in place (advect + enforce_boundary_3D
 // (fluid), WCSPH.py:143-149, sph_base.py:149-179) -- one launch and one pass over the state less.
 #ifndef FORCE_MIN_BLOCKS
-#define FORCE_MIN_BLOCKS 8  // 64 registers: measured best of B in {2,3,4,6} x min-blocks {1,8,10}
+#define FORCE_MIN_BLOCKS 6  // H100 sweep of 6-10 blocks/SM and batch 2 / 4: 6 x batch 4 is fastest (DESIGN.md 3.1)
 #endif
 #ifndef FORCE_BATCH
 #define FORCE_BATCH 4

@@ -1,4 +1,4 @@
-// sph_ptx.cuh -- every line of inline PTX the engine uses, in one place (sm_100a).
+// sph_ptx.cuh -- every line of inline PTX the engine uses, in one place (sm_90a).
 //
 // tests/emu/cuda_emu.h provides host-side stand-ins with the same names, so that the kernel SOURCE in
 // sph_kernels.cuh can also be compiled by g++ and run thread-for-thread under AddressSanitizer
@@ -20,9 +20,11 @@ __device__ __forceinline__ float rcp_ftz(float x) {
     return y;
 }
 
-// one 32-byte record with a single 256-bit read-only load (sm_100: LDG.E.256)
+// one 32-byte record (32-byte aligned, so one sector) as two back-to-back 128-bit read-only loads
+// (sm_90 has no 256-bit LDG; both LDG.E.128 are issued before either result is used)
 __device__ __forceinline__ void ldg256(const float4 *p, float4 &a, float4 &b) {
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.v4.f32 {%4,%5,%6,%7}, [%8+16];"
                  : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
                  : "l"(p));
 }
@@ -35,7 +37,7 @@ __device__ __forceinline__ int ldg_stream(const int32_t *p) {
     return v;
 }
 
-// ---- TMA / mbarrier primitives (sm_90+ PTX, sm_100a SASS: UBLKCP.S.G, SYNCS.ARRIVE.TRANS64) ----
+// ---- TMA / mbarrier primitives (sm_90 PTX; SASS UBLKCP.S.G, SYNCS.ARRIVE.TRANS64) ----
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");

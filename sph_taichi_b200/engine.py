@@ -46,7 +46,7 @@ def make_params(dim, grid_num, particle_radius, density0, stiffness, exponent, d
 class Engine:
     def __init__(self, params, n_max, n_solid=0, n_bodies=0, device=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("sph_taichi_b200 needs a CUDA device: the engine is hand-written sm_100a CUDA "
+            raise RuntimeError("sph_taichi_b200 needs a CUDA device: the engine is hand-written sm_90a CUDA "
                                "with no CPU fallback")
         self.lib = _lib.load()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")

@@ -342,6 +342,8 @@ inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline const char *cudaGetErrorString(cudaError_t) { return "emulated CUDA runtime"; }
 inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16 };
+inline cudaError_t cudaDeviceGetAttribute(int *v, cudaDeviceAttr, int) { *v = 4; return cudaSuccess; }
 inline cudaError_t cudaMemset(void *p, int v, size_t n) { std::memset(p, v, n); return cudaSuccess; }
 inline cudaError_t cudaMemsetAsync(void *p, int v, size_t n, cudaStream_t s) {
     emu::submit(s, [=] { std::memset(p, v, n); });

@@ -1,13 +1,15 @@
-"""Golden vectors from the REFERENCE'S OWN SOURCE (erizmr/SPH_Taichi, /root/reference), executed under the
-pure-Python Taichi stand-in in tests/golden/ti_shim/ (see its docstring for the semantics it implements).
+"""Golden vectors from the REFERENCE'S OWN SOURCE (erizmr/SPH_Taichi, a checkout named by SPH_REFERENCE), executed
+under the pure-Python Taichi stand-in in tests/golden/ti_shim/ (see its docstring for the semantics it implements).
 
-    python tests/golden/make_reference_golden.py          # writes tests/golden/ref_*.npz (+ ref_*_body*.npz)
+    SPH_REFERENCE=<checkout> python tests/golden/make_reference_golden.py          # tests/golden/ref_*.npz (+ ref_*_body*.npz)
+    SPH_REFERENCE=<checkout> python tests/golden/make_reference_golden.py binding  # tests/golden/binding_reference.npz
 
 The reference files particle_system.py / sph_base.py / WCSPH.py / DFSPH.py / config_builder.py are imported
 unmodified; nothing of them is copied into this repository.  Each golden file holds the scene (JSON), the number
 of steps, and the particle fields after `solver.initialize()` and after the last `solver.step()`, in the
 reference's own particle order.  tests/test_golden_reference.py replays the scenes with the CPU oracle.
-This script cannot run on the GPU box (no reference tree there); the vectors are committed.
+`binding` records the input and the per-step trajectory of tests/integration/bind_reference_to_emulated_lib.py.
+The reference is not part of this repository; the vectors are committed.
 """
 import contextlib
 import io
@@ -19,7 +21,7 @@ import tempfile
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = os.environ.get("SPH_REFERENCE", "/root/reference")
+REF = os.environ.get("SPH_REFERENCE")
 
 
 def base_cfg(method=0, dt=0.0004, domain=(0.6, 0.6, 0.6)):
@@ -98,28 +100,66 @@ def snapshot(ps, prefix, out):
         out[prefix + "density_adv"] = ps.density_adv.to_numpy()
 
 
-def run_reference(scene, steps, allow_oob=False):
+def reference_particle_system(scene):
+    if not REF or not os.path.isfile(os.path.join(REF, "particle_system.py")):
+        raise SystemExit("set SPH_REFERENCE to a checkout of erizmr/SPH_Taichi")
     sys.path.insert(0, os.path.join(HERE, "ti_shim"))
     sys.path.insert(0, REF)
-    import taichi as ti
     from config_builder import SimConfig
     from particle_system import ParticleSystem
     fd, path = tempfile.mkstemp(suffix=".json")
     os.write(fd, json.dumps(scene).encode())
     os.close(fd)
+    ps = ParticleSystem(SimConfig(scene_file_path=path), GGUI=False)
+    os.unlink(path)
+    # compile-time constants of the reference's kernels are Python floats (weakly typed), not numpy float64
+    ps.domain_size = [float(v) for v in ps.domain_size]
+    return ps
+
+
+# the scene of tests/integration/bind_reference_to_emulated_lib.py: fluid next to a static block, 6 steps
+BINDING_SCENE = dict(Configuration=base_cfg(),
+                     FluidBlocks=[fluid([0.10, 0.06, 0.10], (6, 7, 6), (0.5, -1.0, 0.0))],
+                     RigidBlocks=[block(1, [0.23, 0.06, 0.10], (3, 5, 6), False)])
+BINDING_STEPS = 6
+BINDING_IN = ("object_id", "x", "x_0", "v", "acceleration", "m_V", "m", "density", "pressure", "material",
+              "is_dynamic", "color", "grid_ids")
+
+
+def run_binding_reference(out_dir):
+    """The reference's fields after solver.initialize() (what a binding packs) and x_0 / x / v / density after each
+    of BINDING_STEPS steps of the reference stepping itself."""
+    out = {}
+    with contextlib.redirect_stdout(io.StringIO()):
+        ps = reference_particle_system(json.loads(json.dumps(BINDING_SCENE)))
+        solver = ps.build_solver()
+        solver.initialize()
+        for f in BINDING_IN:
+            out["init_" + f] = getattr(ps, f).to_numpy()
+        steps = {f: [] for f in ("x_0", "x", "v", "density")}
+        for _ in range(BINDING_STEPS):
+            solver.step()
+            for f in steps:
+                steps[f].append(getattr(ps, f).to_numpy())
+    out.update({"step_" + f: np.stack(v) for f, v in steps.items()})
+    np.savez_compressed(os.path.join(out_dir, "binding_reference.npz"), scene=json.dumps(BINDING_SCENE),
+                        grid_num=np.asarray(ps.grid_num, np.int64), domain_size=np.asarray(ps.domain_size, np.float64),
+                        particle_max_num=ps.particle_max_num, solid_particle_num=ps.solid_particle_num, **out)
+    print("binding particles", ps.particle_max_num, "steps", BINDING_STEPS)
+
+
+def run_reference(scene, steps, allow_oob=False):
     out = {}
     log = io.StringIO()
     with contextlib.redirect_stdout(log):
-        ps = ParticleSystem(SimConfig(scene_file_path=path), GGUI=False)
-        # compile-time constants of the reference's kernels are Python floats (weakly typed), not numpy float64
-        ps.domain_size = [float(v) for v in ps.domain_size]
+        ps = reference_particle_system(scene)
+        import taichi as ti
         solver = ps.build_solver()
         solver.initialize()
         snapshot(ps, "init_", out)
         for _ in range(steps):
             solver.step()
         snapshot(ps, "final_", out)
-    os.unlink(path)
     # Particles resting on an UPPER wall sit in the last cell layer, whose +1 neighbours lie outside the grid: the
     # reference reads them unchecked (SURVEY Q3; harmless on Taichi only because the adjacent memory holds zeros).
     # The stand-in reads such cells as empty -- what the oracle and the engine do by skipping them -- and counts them.
@@ -138,8 +178,11 @@ if __name__ == "__main__":
     args = sys.argv[1:]
     if args[:1] == ["--out"]:
         out_dir, args = args[1], args[2:]
-    names = args or list(SCENES)
+    names = args or list(SCENES) + ["binding"]
     for name in names:
+        if name == "binding":
+            run_binding_reference(out_dir)
+            continue
         scene, steps = SCENES[name]
         out = run_reference(json.loads(json.dumps(scene)), steps, allow_oob=(name in ("wcsph_walls", "wcsph_dambreak")))
         # the oracle / engine side reads rigid bodies from a lattice fixture instead of a mesh

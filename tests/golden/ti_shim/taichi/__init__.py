@@ -1,7 +1,7 @@
 """A pure-Python stand-in for the slice of Taichi that erizmr/SPH_Taichi uses (TEST INFRASTRUCTURE).
 
 Purpose: execute the reference's OWN source files (particle_system.py, sph_base.py, WCSPH.py, DFSPH.py, imported
-unmodified from /root/reference) without the Taichi wheel, so that golden vectors for the CPU oracle come from the
+unmodified from a reference checkout) without the Taichi wheel, so that golden vectors for the CPU oracle come from the
 reference's code rather than from a restatement of it (tests/golden/make_reference_golden.py).
 
 Semantics implemented (what the reference relies on):

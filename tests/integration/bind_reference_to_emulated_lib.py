@@ -1,55 +1,35 @@
-"""INTEGRATION.md section 2, executed: the REFERENCE's ParticleSystem object (its own source, run under the Taichi
-stand-in of tests/golden/ti_shim) is bound to the C ABI of include/sph_b200.h exactly as the stub in INTEGRATION.md
-does -- sph_create on a workspace, then per step sph_pack(fields) / sph_step / sph_unpack(fields) on the reference's
-own field arrays -- and compared, step by step, with a second reference instance that steps itself.
+"""INTEGRATION.md section 2, executed: the REFERENCE's ParticleSystem fields (its own source, run under the Taichi
+stand-in of tests/golden/ti_shim, stored in tests/golden/binding_reference.npz) are bound to the C ABI of
+include/sph_b200.h exactly as the stub in INTEGRATION.md does -- sph_create on a workspace, then per step
+sph_pack(fields) / sph_step / sph_unpack(fields) on field arrays of the reference's layout -- and compared, step by
+step, with the trajectory of the reference stepping itself (same file, written by
+tests/golden/make_reference_golden.py).
 
 The library is the host-emulated build of the same sources (tests/emu/), so this runs without a GPU; "device
-pointers" are host pointers.  Prints one JSON line.  TEST INFRASTRUCTURE (needs /root/reference).
+pointers" are host pointers.  Prints one JSON line.
 
     SPH_B200_LIB=tests/emu/_build/libsph_b200_emu.so python tests/integration/bind_reference_to_emulated_lib.py
 """
-import contextlib
 import ctypes as C
-import io
 import json
 import os
 import sys
-import tempfile
+from types import SimpleNamespace
 
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden", "ti_shim"))
-sys.path.insert(0, os.environ.get("SPH_REFERENCE", "/root/reference"))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
-from make_reference_golden import base_cfg, block, fluid  # noqa: E402  (scene helpers only)
-
-STEPS = 6
-scene = dict(Configuration=base_cfg(),
-             FluidBlocks=[fluid([0.10, 0.06, 0.10], (6, 7, 6), (0.5, -1.0, 0.0))],
-             RigidBlocks=[block(1, [0.23, 0.06, 0.10], (3, 5, 6), False)])
-
-
-def reference_instance():
-    from config_builder import SimConfig
-    from particle_system import ParticleSystem
-    fd, path = tempfile.mkstemp(suffix=".json")
-    os.write(fd, json.dumps(scene).encode())
-    os.close(fd)
-    ps = ParticleSystem(SimConfig(scene_file_path=path), GGUI=False)
-    os.unlink(path)
-    ps.domain_size = [float(v) for v in ps.domain_size]
-    solver = ps.build_solver()
-    solver.initialize()
-    return ps, solver
-
-
-with contextlib.redirect_stdout(io.StringIO()):
-    ps, solver = reference_instance()      # bound to the library below
-    twin, twin_solver = reference_instance()  # steps itself
+gold = np.load(os.path.join(ROOT, "tests", "golden", "binding_reference.npz"))
+scene = json.loads(str(gold["scene"]))
+STEPS = len(gold["step_x"])
+# the reference's field arrays after solver.initialize(), each wrapped like a Taichi field's `.data`
+ps = SimpleNamespace(grid_num=gold["grid_num"], domain_size=[float(v) for v in gold["domain_size"]],
+                     particle_max_num=int(gold["particle_max_num"]), solid_particle_num=int(gold["solid_particle_num"]),
+                     **{k[5:]: SimpleNamespace(data=np.ascontiguousarray(gold[k])) for k in gold.files
+                        if k.startswith("init_")})
 
 # ---- the binding of INTEGRATION.md section 2 ----
 from sph_taichi_b200 import _lib, engine  # noqa: E402  (parameter struct + argtypes only; no CUDA involved)
@@ -92,11 +72,9 @@ for step in range(STEPS):
     assert lib.sph_pack(ctx, C.byref(f), n, None) == 0, lib.sph_last_error(ctx)
     assert lib.sph_step(ctx, 1, None) == 0, lib.sph_last_error(ctx)
     assert lib.sph_unpack(ctx, C.byref(f), None) == 0, lib.sph_last_error(ctx)
-    with contextlib.redirect_stdout(io.StringIO()):
-        twin_solver.step()
-    same_order &= bool(np.array_equal(ps.x_0.data, twin.x_0.data))
+    same_order &= bool(np.array_equal(ps.x_0.data, gold["step_x_0"][step]))
     for k in worst:
-        a, b = getattr(ps, k).data.astype(np.float64), getattr(twin, k).data.astype(np.float64)
+        a, b = getattr(ps, k).data.astype(np.float64), gold["step_" + k][step].astype(np.float64)
         worst[k] = max(worst[k], float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)))
 lib.sph_destroy(ctx)
 print(json.dumps({"particles": int(n), "steps": STEPS, "same_particle_order": same_order, "max_rel_err": worst}))

@@ -3,8 +3,8 @@ on the CPU, run a subset of the `gpu` parity tests (the same test functions, the
 tolerances) -- once plain and once under AddressSanitizer.
 
 This is a check of the kernel and host SOURCE (index arithmetic, staging windows, list layout, launch
-sequences, graph capture), not of the sm_100a binary: the B200 runs of the `gpu` marker remain the parity
-gate.  The product library is never involved; the emulated build lives in tests/emu/_build/."""
+sequences, graph capture), not of the sm_90a binary: the H100 runs of the `gpu` marker remain the parity
+check.  The product library is never involved; the emulated build lives in tests/emu/_build/."""
 import os
 import re
 import subprocess

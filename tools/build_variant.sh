@@ -4,5 +4,5 @@ set -e
 cd "$(dirname "$0")/.."
 name=$1; shift
 mkdir -p build_exp
-nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -shared -Xcompiler -fPIC "$@" \
+nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -shared -Xcompiler -fPIC "$@" \
   -o build_exp/libsph_$name.so sph_taichi_b200/csrc/sph_b200.cu

@@ -1,7 +1,7 @@
 """dram__bytes_read.sum + dram__bytes_write.sum per launch of the two pair kernels from an `ncu --set full` capture
 -> profiles/dram_traffic.json (what bench.py reports as roofline.traffic).
 
-    python tools/ncu_dram_traffic.py gpurun_out/prof_r02_final.ncu-rep dragon_bath profiles/r02_final_pair_kernels_ncu.txt
+    python tools/ncu_dram_traffic.py prof.ncu-rep dragon_bath profiles/pair_kernels_ncu.txt
 """
 import csv, io, json, os, subprocess, sys
 

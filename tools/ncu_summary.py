@@ -1,6 +1,6 @@
 """Summarise an .ncu-rep (ncu --set full) into a small text table for profiles/.
 
-    python tools/ncu_summary.py gpurun_out/prof_v2.ncu-rep > profiles/r01_v2_pair_kernels.txt
+    python tools/ncu_summary.py prof.ncu-rep > profiles/pair_kernels_ncu.txt
 """
 import csv
 import io
