@@ -43,6 +43,8 @@ extern "C" {
 #define SPH_STATUS_BAD_POLAR 2u   /* shape matching hit a singular A */
 #define SPH_STATUS_HALO_CAPACITY 4u  /* sharded: a send range exceeded halo_capacity (records were cut off) */
 #define SPH_STATUS_SHARD_CAPACITY 8u /* sharded: live + received records ran into the receive regions */
+#define SPH_STATUS_SHARD_VELOCITY 16u /* sharded DFSPH: a particle moved >= one cell layer in x in one step */
+#define SPH_STATUS_GHOST_ALIGN 32u   /* sharded DFSPH: a neighbour's boundary layers and the ghost layers differ */
 
 /* Scalar parameters.  All constants are folded in double on the host exactly as the
  * reference folds them in Python scope before Taichi bakes them into kernels
@@ -209,9 +211,18 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
  * most one layer every `rebalance_every` steps, decided identically on both sides of a cut from the owned
  * counts in the headers.  Fluid-only scenes with one fluid (uniform masses); rigid bodies are single-GPU.
  *
+ * DFSPH contexts (sph_set_dfsph(1) before sph_shard_configure) step with sph_shard_dfsph_step instead: the same
+ * classification, sort, re-balancing and end-of-step record exchange, plus a once-per-step ghost alignment (each
+ * rank overwrites its ghost layers with the neighbour's owned boundary layers in the neighbour's sorted order) and
+ * small exchanges of the outermost owned layer's velocities / {factor, density_adv} whenever the owner changes them
+ * -- two per Jacobi sweep.  The loops' error sums are all-gathered and added in rank order, so every rank takes the
+ * same convergence decision and issues the same transport calls.
+ *
+ *
  * The exchange goes through an SphTransport: NCCL point-to-point (libnccl.so.2 is dlopen'ed; the communicator
  * belongs to this library, created from an id the caller distributes), or caller-supplied functions (the CPU
- * test-suite routes them to torch.distributed / gloo against the host-emulated build). */
+ * test-suite routes them to torch.distributed / gloo against the host-emulated build); set it before
+ * sph_shard_configure. */
 typedef struct SphTransport {
     void *user;
     int (*group_start)(void *user);
@@ -232,6 +243,16 @@ int sph_shard_begin(SphCtx *ctx, void *stream);
 /* nsteps sharded SPHBase.step()s (sph_base.py:263-271): asynchronous launches that run ahead of the device (no host
  * synchronisation inside a step); SPH_SHARD_GRAPH=1 replays one captured CUDA graph per step instead */
 int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream);
+/* nsteps sharded DFSPH SPHBase.step()s (sph_base.py:263-271 with DFSPH.substep, DFSPH.py:399-408) of a fluid-only
+ * DFSPH context: the step of sph_dfsph_step with `io` used the same way, except that io->n_fluid is the GLOBAL fluid
+ * count (all ranks).  Every rank returns the same iterations, first_batch and avg_err values.  Eager launches with
+ * one host wait per batch of Jacobi sweeps, like sph_dfsph_step (SPH_SHARD_GRAPH does not apply).  A particle that
+ * moves a whole cell layer in x in one step sets SPH_STATUS_SHARD_VELOCITY (the record exchange would lose it);
+ * sph_shard_info reports the status word. */
+int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
+/* out2 = {transport groups this context issued from the host, bytes it sent in them}; graph replays of
+ * sph_shard_step (SPH_SHARD_GRAPH=1) re-issue the captured groups without counting them */
+int sph_shard_transport_stats(SphCtx *ctx, uint64_t *out2);
 /* the exchange alone: sends the packed staging, receives behind the live records (SURVEY.md section 8b) */
 int sph_halo_exchange(SphCtx *ctx, void *stream);
 /* synchronising read of the device-resident step state: out16 = {n_live, owned, x_lo, x_hi, step, own_begin,

@@ -26,7 +26,8 @@ ABI_SYMBOLS = [
     "sph_solve_constraints", "sph_get_rigid_state", "sph_step", "sph_read_status", "sph_clear_status", "sph_neighbor_stats", "sph_particle_count",
     "sph_launch_count", "sph_profile_step", "sph_timer_name", "sph_state_offsets", "sph_set_dfsph", "sph_dfsph_op", "sph_dfsph_solve", "sph_dfsph_step",
     "sph_comm_unique_id", "sph_comm_init_nccl", "sph_comm_set_transport", "sph_shard_configure", "sph_shard_begin",
-    "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step",
+    "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step", "sph_shard_dfsph_step",
+    "sph_shard_transport_stats",
 ]
 
 
@@ -157,6 +158,8 @@ def load():
         "sph_halo_exchange": (C.c_int, [vp, vp]),
         "sph_shard_info": (C.c_int, [vp, C.POINTER(i32), C.POINTER(u64), vp]),
         "sph_shard_profile_step": (C.c_int, [vp, C.POINTER(C.c_float), vp]),
+        "sph_shard_dfsph_step": (C.c_int, [vp, i32, C.POINTER(SphDfsphStep), vp]),
+        "sph_shard_transport_stats": (C.c_int, [vp, C.POINTER(u64)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

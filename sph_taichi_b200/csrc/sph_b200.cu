@@ -154,6 +154,10 @@ struct SphCtx {
     // second density launch can cost more than it hides (not measured on H100s)
     bool split_density = false;
     int64_t shard_sequences = 0;  // sequences run so far (begin = 0): sequence q feeds the plan kernel of q + 1
+    // sharded DFSPH: records per side of the ghost alignment (sgw layers) and of a per-sweep exchange (one layer)
+    int32_t align_cap = 0, sweep_cap = 0;
+    int shard_world = 1;  // world size the shard buffer's per-rank error partials were sized for
+    uint64_t xfer_groups = 0, xfer_bytes = 0;  // transport groups issued from the host, and the bytes this rank sent
 };
 
 namespace {
@@ -300,9 +304,10 @@ int launch_neighbor_build(SphCtx *c, cudaStream_t st, StageTimer *tm, int64_t *k
 
 // density + neighbour lists, then forces (+ integration).  SPH_DENSITY_VARIANT / SPH_FORCE_VARIANT = 0
 // select the ablation variants (second dense loop for the density sum; separate advect kernel).
-void launch_pair_density(SphCtx *c, cudaStream_t st, int64_t *kernels, int split_mode = 0) {
+// n_grid (sharded DFSPH): the grid covers [0, n_grid) instead of all P.n slots
+void launch_pair_density(SphCtx *c, cudaStream_t st, int64_t *kernels, int split_mode = 0, int64_t n_grid = -1) {
     const DevParams &P = c->P;
-    const int blocks = blocks_for(P.n, DENS_WARPS * 32);
+    const int blocks = blocks_for(n_grid < 0 ? P.n : n_grid, DENS_WARPS * 32);
     if (c->var_density == 0) PDL_LAUNCH((k_density_tma<false, false>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
     else if (P.dfsph || c->var_density == 2) PDL_LAUNCH((k_density_tma<true, false>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
     else PDL_LAUNCH((k_density_tma<true, true>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
@@ -751,9 +756,11 @@ int shard_exchange(SphCtx *c, cudaStream_t st, bool wide) {
     const uint64_t bytes = (uint64_t)(wide ? c->P.halo_cap : c->narrow_cap) * 16;
     float4 *cur[4] = {S.posm, S.veld, S.x0id, S.misc};
     TRANSPORT_OP(st, t.group_start(t.user));
+    c->xfer_groups += 1;
     for (int side = 0; side < 2; ++side) {
         const int peer = side == 0 ? c->rank - 1 : c->rank + 1;
         if (peer < 0 || peer >= c->world) continue;
+        c->xfer_bytes += 4 * bytes + 64;
         const int64_t tail = (int64_t)c->P.n - (side == 0 ? 2 : 1) * (int64_t)c->P.halo_cap;
         for (int k = 0; k < 4; ++k) {
             const void *sp = S.stage[side][k];
@@ -903,15 +910,17 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
     if (!ctx->bodies.empty() || ctx->P.n_solid > 0)
         return fail(ctx, SPH_E_ARG, "x-slab sharding supports fluid-only scenes (rigid bodies are single-GPU, SURVEY 8e)");
-    if (!ctx->P.uniform_fluid || ctx->P.dfsph)
-        return fail(ctx, SPH_E_ARG, "x-slab sharding needs the uniform-fluid WCSPH step (one fluid density)");
+    if (!ctx->P.uniform_fluid)
+        return fail(ctx, SPH_E_ARG, "x-slab sharding needs a single fluid density (uniform fluid masses)");
     if (halo_capacity < 1 || 2 * halo_capacity + ctx->P.n > ctx->n_max)
         return fail(ctx, SPH_E_CAPACITY, "capacity: packed particles + 2 * halo_capacity receive slots exceed n_max");
     if (rebalance_every < 0) return SPH_E_ARG;
     const int32_t n_mine = ctx->P.n;
     drop_graphs(ctx);
     if (ctx->shard_buf) { cudaFree(ctx->shard_buf); ctx->shard_buf = nullptr; }
-    const uint64_t bytes = 256 + 2 * 256 + 8 * align_up((uint64_t)halo_capacity * 16, 256);
+    // {state ints | 2 headers | staging | DFSPH: DX ranges + alignment headers | one fp64 error partial per rank}
+    const uint64_t bytes = 256 + 2 * 256 + 8 * align_up((uint64_t)halo_capacity * 16, 256) + 256 +
+                           align_up((uint64_t)ctx->world * 8, 256);
     CUDA_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->shard_buf), bytes));
     CUDA_TRY(ctx, cudaMemset(ctx->shard_buf, 0, bytes));
     int32_t sd[SD_INTS] = {0};
@@ -921,6 +930,10 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
     ctx->P.has_left = ctx->rank > 0; ctx->P.has_right = ctx->rank + 1 < ctx->world;
     ctx->P.rebalance_every = rebalance_every;
     ctx->narrow_cap = (int32_t)((halo_capacity * (ghost_layers + 1) + ghost_layers + 1) / (ghost_layers + 2));
+    // halo_capacity covers ghost_layers + 2 layers: the alignment carries ghost_layers of them, a sweep one
+    ctx->align_cap = (int32_t)((halo_capacity * ghost_layers + ghost_layers + 1) / (ghost_layers + 2));
+    ctx->sweep_cap = (int32_t)((halo_capacity + ghost_layers + 1) / (ghost_layers + 2));
+    ctx->shard_world = ctx->world;
     ctx->shard_sequences = 0;
     ctx->split_density = ctx->world > 4;
     if (const char *v = std::getenv("SPH_SHARD_SPLIT_DENSITY")) ctx->split_density = std::atoi(v) != 0;
@@ -967,6 +980,7 @@ int sph_halo_exchange(SphCtx *ctx, void *stream) {
 int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream) {
     REQUIRE_SHARD(ctx);
     if (nsteps < 0) return SPH_E_ARG;
+    if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_step is the WCSPH step; DFSPH contexts step with sph_shard_dfsph_step");
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // Un-graphed launches are the DEFAULT here: nothing in a sharded step waits for the host any more, so the launches
@@ -1015,6 +1029,7 @@ int sph_shard_info(SphCtx *ctx, int32_t *out16, uint64_t *out_sent, void *stream
 int sph_shard_profile_step(SphCtx *ctx, float *ms_out6, void *stream) {
     REQUIRE_SHARD(ctx);
     if (!ms_out6) return SPH_E_ARG;
+    if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_profile_step times the WCSPH step");
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaEvent_t ev[8];
@@ -1086,29 +1101,115 @@ int sph_dfsph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream
 }  // extern "C"
 namespace {
 
+// Sharded DFSPH blocks of the shard buffer, behind the staging: the DX_* ranges + alignment headers (256 B), then one
+// fp64 error partial per rank
+inline int32_t *shard_dx(const SphCtx *c) {
+    return reinterpret_cast<int32_t *>(c->shard_buf + 768 + 8 * align_up((uint64_t)c->P.halo_cap * 16, 256));
+}
+inline double *shard_err_parts(const SphCtx *c) { return reinterpret_cast<double *>(shard_dx(c) + DX_INTS); }
+
+// One exchange of the sharded DFSPH step with both neighbours: pack -> one transport group -> unpack.
+//   DX_ALIGN: the ghost alignment (4 record arrays of the sgw boundary layers + a 16-byte header per side), received
+//             into the receive regions behind the live records, which stay unused until the end-of-step exchange;
+//   DX_VELD / DX_DFS: one 16-byte word per particle of the outermost owned layer, received into the second staging
+//             array.
+// Fixed-size messages (align_cap / sweep_cap records), so both sides always agree on the byte counts.  gather_err: the
+// same group also sends this rank's fp64 error partial (ctrl->err) to every other rank and receives theirs into
+// shard_err_parts() -- an all-gather of 8 bytes with plain send / recv.  ctrl (may be NULL): the pack and unpack of a
+// sweep behind the converged one return at once, but its transport calls are still issued, so that every rank issues
+// the same sequence.
+int shard_dfsph_exchange(SphCtx *c, cudaStream_t st, int what, DfsphCtrl *ctrl, bool gather_err, int64_t *kernels) {
+    if (c->world <= 1) return SPH_OK;
+    if (!c->has_transport) return fail(c, SPH_E_ARG, "no transport: call sph_comm_init_nccl or sph_comm_set_transport first");
+    const SphTransport t = c->transport;
+    const DevArrays S = c->S;
+    const DevParams &P = c->P;
+    int32_t *dx = shard_dx(c);
+    double *parts = shard_err_parts(c);
+    const int cap = what == DX_ALIGN ? c->align_cap : c->sweep_cap;
+    const uint64_t bytes = (uint64_t)cap * 16;
+    const int narr = what == DX_ALIGN ? 4 : 1;
+    float4 *cur[4] = {S.posm, S.veld, S.x0id, S.misc};
+    float4 *rec[2][4];
+    for (int side = 0; side < 2; ++side)
+        for (int k = 0; k < 4; ++k)
+            rec[side][k] = what == DX_ALIGN ? cur[k] + ((int64_t)P.n - (2 - side) * (int64_t)P.halo_cap) : S.stage[side][1];
+    const dim3 grid(blocks_for(cap, 256), 2);
+    k_dfsph_shard_pack<<<grid, 256, 0, st>>>(P, S, dx, what, ctrl);
+    CUDA_TRY(c, cudaGetLastError());
+    TRANSPORT_OP(st, t.group_start(t.user));
+    c->xfer_groups += 1;
+    for (int side = 0; side < 2; ++side) {
+        const int peer = side == 0 ? c->rank - 1 : c->rank + 1;
+        if (peer < 0 || peer >= c->world) continue;
+        for (int k = 0; k < narr; ++k) {
+            const void *sp = S.stage[side][k];
+            void *rp = rec[side][k];
+            TRANSPORT_OP(st, t.send(t.user, sp, bytes, peer, st));
+            TRANSPORT_OP(st, t.recv(t.user, rp, bytes, peer, st));
+        }
+        c->xfer_bytes += narr * bytes;
+        if (what == DX_ALIGN) {
+            const void *hs = dx + DX_HDR_SEND + 4 * side;
+            void *hr = dx + DX_HDR_RECV + 4 * side;
+            TRANSPORT_OP(st, t.send(t.user, hs, 16, peer, st));
+            TRANSPORT_OP(st, t.recv(t.user, hr, 16, peer, st));
+            c->xfer_bytes += 16;
+        }
+    }
+    if (gather_err) {
+        for (int r = 0; r < c->world; ++r) {
+            if (r == c->rank) continue;
+            const void *es = &ctrl->err;
+            void *er = parts + r;
+            TRANSPORT_OP(st, t.send(t.user, es, 8, r, st));
+            TRANSPORT_OP(st, t.recv(t.user, er, 8, r, st));
+            c->xfer_bytes += 8;
+        }
+    }
+    TRANSPORT_OP(st, t.group_end(t.user, st));
+    k_dfsph_shard_unpack<<<grid, 256, 0, st>>>(P, S, dx, what, ctrl, rec[0][0], rec[0][1], rec[0][2], rec[0][3], rec[1][0],
+                                               rec[1][1], rec[1][2], rec[1][3]);
+    *kernels += 2;
+    CUDA_TRY(c, cudaGetLastError());
+    return SPH_OK;
+}
+
 // The Jacobi loop of divergence_solve (mode 0, DFSPH.py:245-254) or pressure_solve (mode 1, DFSPH.py:323-331) with the
 // loop condition on the device: sweeps are launched in batches (the first as long as the caller expects the loop to
 // run -- the previous step's count is a good guess), every sweep ends with k_dfsph_check, sweeps behind the
 // converged one return at once, and the host reads the control block once per batch.
+// Sharded (P.slab_on): every sweep also sends the owned boundary layer's velocities after the iteration and its
+// {factor, density_adv} after the density change to the neighbours' first ghost layer, and all-gathers the error
+// partials for k_dfsph_check_ranked; n_fluid is then the global fluid count.
 int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, float offset, int64_t n_fluid,
-                     int32_t first_batch, DfsphCtrl *h, cudaStream_t st) {
+                     int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t n_grid = -1) {
     const DevParams &P = ctx->P;
     DfsphCtrl *ctrl = reinterpret_cast<DfsphCtrl *>(ctx->ws + ctx->L.off_scratch);
     *h = DfsphCtrl{};
     CUDA_TRY(ctx, cudaMemsetAsync(ctrl, 0, sizeof(DfsphCtrl), st));
     if (P.n == 0) return SPH_OK;
-    const int b128 = blocks_for(P.n, 128);
+    const bool shard = P.slab_on != 0;
+    const int b128 = blocks_for(n_grid < 0 ? P.n : n_grid, 128);
     int batch = std::max(1, std::min(first_batch, 64));
     while (!h->done) {
         for (int s = 0; s < batch; ++s) {
-            if (mode == 0) {
-                k_dfsph_iteration<0><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
-                k_dfsph_density_change_err<0><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
-            } else {
-                k_dfsph_iteration<1><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
-                k_dfsph_density_change_err<1><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
+            if (mode == 0) k_dfsph_iteration<0><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+            else k_dfsph_iteration<1><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+            if (shard) {
+                int rc = shard_dfsph_exchange(ctx, st, DX_VELD, ctrl, false, &ctx->launches);
+                if (rc) return rc;
             }
-            k_dfsph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
+            if (mode == 0) k_dfsph_density_change_err<0><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
+            else k_dfsph_density_change_err<1><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
+            if (shard) {
+                int rc = shard_dfsph_exchange(ctx, st, DX_DFS, ctrl, true, &ctx->launches);
+                if (rc) return rc;
+                k_dfsph_check_ranked<<<1, 1, 0, st>>>(ctrl, shard_err_parts(ctx), ctx->rank, ctx->world, (double)n_fluid, eta,
+                                                      max_iterations);
+            } else {
+                k_dfsph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
+            }
         }
         ctx->launches += 3 * (int64_t)batch;
         CUDA_TRY(ctx, cudaGetLastError());
@@ -1116,6 +1217,80 @@ int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, 
         CUDA_TRY(ctx, cudaStreamSynchronize(st));
         batch = 2;  // the guess was short: continue in pairs
     }
+    return SPH_OK;
+}
+
+// One sharded DFSPH SPHBase.step() (fluid only; no overlap of the exchanges with computation):
+//   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> densities (owned + first ghost layer) -> factor
+//   -> [density change -> * 1/dt -> dfs exchange -> divergence loop -> * dt] -> non-pressure forces -> predict velocity
+//   -> veld exchange -> density_adv -> * 1/dt^2 -> dfs exchange -> pressure loop -> advect + clamp (owned)
+//   -> pack the send ranges -> the record exchange that feeds the next step's classification
+// After the alignment a ghost record holds exactly what its owner holds in the same position, so a value that changes
+// on the owner is sent once per change -- veld after each Jacobi iteration and after predict_velocity, dfs after each
+// density change -- and every pass reads current ghost values.  The {factor, density_adv} words are sent AFTER the
+// multiply_time_step that follows each loop's opening density change: one message carries both, and the scale at the
+// end of the divergence loop needs no message because nothing reads a ghost's factor before the pressure loop's
+// opening exchange.
+int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, SphDfsphStep *io, bool wide, int64_t *kernels) {
+    k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+    int rc = launch_neighbor_build(c, st, nullptr, kernels, /*move_acc=*/false);
+    if (rc) return rc;
+    const DevParams &P = c->P;  // after the build: the array binding changed sides
+    k_shard_info<<<1, 32, 0, st>>>(P, c->S, P.sgw + (wide ? 2 : 1), wide ? P.halo_cap : c->narrow_cap);
+    k_dfsph_shard_ranges<<<1, 32, 0, st>>>(P, c->S, shard_dx(c), c->align_cap, c->sweep_cap);
+    *kernels += 2;
+    CUDA_TRY(c, cudaGetLastError());
+    rc = shard_dfsph_exchange(c, st, DX_ALIGN, nullptr, false, kernels);
+    if (rc) return rc;
+    // The step waits on the host once per batch of sweeps anyway; one more short wait here for the live count lets
+    // every DFSPH launch cover [0, n_live) -- owned records and ghosts -- instead of the whole capacity.
+    int32_t n_live = 0;
+    CUDA_TRY(c, cudaMemcpyAsync(&n_live, c->S.sd + SD_N_LIVE, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(c, cudaStreamSynchronize(st));
+    const int64_t n_grid = std::min<int64_t>(std::max<int32_t>(n_live, 1), P.n);
+    const int b128 = blocks_for(n_grid, 128), b256 = blocks_for(n_grid, 256);
+    // substep (DFSPH.py:399-408)
+    launch_pair_density(c, st, kernels, /*split_mode=*/0, n_grid);
+    c->list_valid = true;
+    k_dfsph_factor<<<b128, 128, 0, st>>>(P, c->S);
+    *kernels += 1;
+    DfsphCtrl h{};
+    if (io->enable_divergence_solver) {  // divergence_solve, DFSPH.py:236-276
+        k_dfsph_density_change<0><<<b128, 128, 0, st>>>(P, c->S);
+        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt);
+        *kernels += 2;
+        rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
+        if (rc) return rc;
+        rc = dfsph_solve_loop(c, 0, io->max_iterations_v, io->eta_v, 0.0f, io->n_fluid, io->first_batch_v, &h, st, n_grid);
+        if (rc) return rc;
+        io->iterations_v = h.iterations; io->avg_err_v = h.last_avg; io->first_batch_v = std::max(1, h.sweeps);
+        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->dt);
+        *kernels += 1;
+    }
+    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(P, c->S);
+    k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, c->S);
+    *kernels += 2;
+    rc = shard_dfsph_exchange(c, st, DX_VELD, nullptr, false, kernels);
+    if (rc) return rc;
+    // pressure_solve, DFSPH.py:314-352
+    k_dfsph_density_change<1><<<b128, 128, 0, st>>>(P, c->S);
+    k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt2);
+    *kernels += 2;
+    rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
+    if (rc) return rc;
+    rc = dfsph_solve_loop(c, 1, io->max_iterations, io->eta, io->density0, io->n_fluid, io->first_batch, &h, st, n_grid);
+    if (rc) return rc;
+    io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
+    k_dfsph_advect<<<b256, 256, 0, st>>>(P, c->S);
+    k_enforce_boundary<<<b256, 256, 0, st>>>(P, c->S, /*particle_type=*/1);  // enforce_boundary_3D(fluid), sph_base.py:271
+    // the advanced records of the send ranges -> staging, then the exchange the next step classifies
+    k_shard_apply<<<dim3(blocks_for(P.halo_cap, 256), 2), 256, 0, st>>>(P, c->S, /*copy_all=*/1);
+    *kernels += 3;
+    CUDA_TRY(c, cudaGetLastError());
+    rc = shard_exchange(c, st, wide);
+    if (rc) return rc;
+    c->built = false; c->list_valid = false;
     return SPH_OK;
 }
 
@@ -1140,7 +1315,7 @@ int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double et
 int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) {
     if (!ctx || !io || nsteps < 0 || io->n_fluid < 1) return SPH_E_ARG;
     if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called");
-    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, "DFSPH is single-GPU");
+    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, "this context is sharded: step it with sph_shard_dfsph_step");
     if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int s = 0; s < nsteps; ++s) {
@@ -1184,6 +1359,29 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) 
         ctx->launches += 1;
         CUDA_TRY(ctx, cudaGetLastError());
     }
+    return SPH_OK;
+}
+
+int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) {
+    REQUIRE_SHARD(ctx);
+    if (!io || nsteps < 0 || io->n_fluid < 1) return SPH_E_ARG;
+    if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called: WCSPH contexts step with sph_shard_step");
+    if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
+    if (ctx->world != ctx->shard_world)
+        return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure: configure again");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int s = 0; s < nsteps; ++s) {
+        int rc = shard_dfsph_sequence(ctx, st, io, shard_wide(ctx), &ctx->launches);
+        if (rc) return rc;
+        ctx->shard_sequences += 1;
+    }
+    return SPH_OK;
+}
+
+int sph_shard_transport_stats(SphCtx *ctx, uint64_t *out2) {
+    if (!ctx || !out2) return SPH_E_ARG;
+    out2[0] = ctx->xfer_groups;
+    out2[1] = ctx->xfer_bytes;
     return SPH_OK;
 }
 

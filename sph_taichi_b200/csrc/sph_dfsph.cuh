@@ -65,8 +65,15 @@ __device__ __forceinline__ void for_listed_neighbors(const DevParams &P, const D
     }
 }
 
-__device__ __forceinline__ bool dfsph_fluid(const DevParams &P, const DevArrays &S, int i, uint32_t &fl) {
+// x-slab sharding: P.n is the capacity, and every per-particle DFSPH kernel but the density pass works on the
+// owned index range of the device step state only (ghosts are neighbours; their values come from the owner)
+__device__ __forceinline__ bool dfsph_in_range(const DevParams &P, const DevArrays &S, int i) {
     if (i >= P.n) return false;
+    return !P.slab_on || (i >= S.sd[SD_OWN0] && i < S.sd[SD_OWN1]);
+}
+
+__device__ __forceinline__ bool dfsph_fluid(const DevParams &P, const DevArrays &S, int i, uint32_t &fl) {
+    if (!dfsph_in_range(P, S, i)) return false;
     fl = __float_as_uint(S.misc[i].z);
     return (fl & FLAG_FLUID) != 0;
 }
@@ -156,9 +163,9 @@ __global__ void __launch_bounds__(128) k_dfsph_density_change_err(DevParams P, D
 
 // The loop condition of divergence_solve / pressure_solve (DFSPH.py:245-254, 323-331), evaluated on the device:
 //   while m < 1 or m < max_iterations:  avg = sweep();  if avg <= eta: break;  m += 1
-__global__ void k_dfsph_check(DfsphCtrl *ctrl, double n_fluid, double eta, int32_t max_iterations) {
-    if (ctrl->done) return;
-    const double avg = ctrl->err / n_fluid;
+__device__ __forceinline__ void dfsph_check_sum(DfsphCtrl *ctrl, double err, double n_fluid, double eta,
+                                                int32_t max_iterations) {
+    const double avg = err / n_fluid;
     ctrl->last_avg = avg;
     ctrl->err = 0.0;
     ctrl->sweeps += 1;
@@ -166,6 +173,20 @@ __global__ void k_dfsph_check(DfsphCtrl *ctrl, double n_fluid, double eta, int32
     const int32_t m = ctrl->iterations + 1;
     ctrl->iterations = m;
     if (!(m < 1 || m < max_iterations)) ctrl->done = 1;
+}
+__global__ void k_dfsph_check(DfsphCtrl *ctrl, double n_fluid, double eta, int32_t max_iterations) {
+    if (ctrl->done) return;
+    dfsph_check_sum(ctrl, ctrl->err, n_fluid, eta, max_iterations);
+}
+// Sharded variant: parts[r] holds rank r's error partial (this rank's own is still in ctrl->err), all-gathered over
+// the transport.  The partials are summed in RANK order, so every rank computes bit-identical avg / done / iterations
+// and issues the same number of transport calls.
+__global__ void k_dfsph_check_ranked(DfsphCtrl *ctrl, const double *parts, int32_t rank, int32_t world, double n_fluid,
+                                     double eta, int32_t max_iterations) {
+    if (ctrl->done) return;
+    double err = rank == 0 ? ctrl->err : parts[0];
+    for (int r = 1; r < world; ++r) err += r == rank ? ctrl->err : parts[r];
+    dfsph_check_sum(ctrl, err, n_fluid, eta, max_iterations);
 }
 
 // DFSPH.py:221-227
@@ -235,7 +256,7 @@ __global__ void __launch_bounds__(128) k_dfsph_iteration(DevParams P, DevArrays 
 // compute_non_pressure_forces (DFSPH.py:50-101): cohesion + viscosity, list based
 __global__ void __launch_bounds__(128) k_dfsph_non_pressure(DevParams P, DevArrays S) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= P.n) return;
+    if (!dfsph_in_range(P, S, i)) return;
     float4 mi = S.misc[i];
     uint32_t fl = __float_as_uint(mi.z);
     if (!(fl & FLAG_FLUID)) {
@@ -274,10 +295,11 @@ __global__ void k_dfsph_predict_velocity(DevParams P, DevArrays S) {
     S.veld[i] = v;
 }
 
-// DFSPH.py:104-111
+// DFSPH.py:104-111.  Sharded: the end-of-step exchange only carries the cell layers next to a cut, so a particle
+// that moves a whole cell layer in x within one step could be lost -- flagged instead (SPH_STATUS_SHARD_VELOCITY).
 __global__ void k_dfsph_advect(DevParams P, DevArrays S) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= P.n) return;
+    if (!dfsph_in_range(P, S, i)) return;
     uint32_t fl = __float_as_uint(S.misc[i].z);
     if (!(fl & FLAG_DYNAMIC)) return;
     float4 p = S.posm[i], v = S.veld[i];
@@ -286,6 +308,125 @@ __global__ void k_dfsph_advect(DevParams P, DevArrays S) {
         v.x += P.dt * a.x; v.y += P.dt * a.y; v.z += P.dt * a.z;
         S.veld[i] = v;
     }
+    if (P.slab_on && !(fabsf(v.x) * P.dt < P.h)) atomicOr(S.status, SPH_STATUS_SHARD_VELOCITY);
     p.x += P.dt * v.x; p.y += P.dt * v.y; p.z += P.dt * v.z;
     S.posm[i] = p;
+}
+
+// ---- x-slab sharding of the DFSPH step (sph_shard_dfsph_step) ----------------------------------------------------
+// Index ranges of the sorted arrays that the per-step ghost alignment and the per-sweep exchanges work on
+// (DevArrays::sd holds the WCSPH step state; these live in a separate block of the shard buffer).
+enum {
+    DX_SEND_L0 = 0, DX_SEND_L1, DX_SEND_L1E,  // to the left: owned layers [sx0, sx0 + sgw), the first ends at L1E
+    DX_SEND_R0, DX_SEND_R1, DX_SEND_R1B,      // to the right: owned layers [sx1 - sgw, sx1), the last starts at R1B
+    DX_GHOST_L0, DX_GHOST_L1, DX_GHOST_L1B,   // ghost layers [sx0 - sgw, sx0), the first ghost layer starts at L1B
+    DX_GHOST_R0, DX_GHOST_R1, DX_GHOST_R1E,   // ghost layers [sx1, sx1 + sgw), the first ghost layer ends at R1E
+    DX_HDR_SEND = 16,                         // 4 ints per side: {records of the sgw layers, records of the first}
+    DX_HDR_RECV = 32,                         // the same, received from the left / right neighbour
+    DX_INTS = 64
+};
+enum { DX_ALIGN = 0, DX_VELD = 1, DX_DFS = 2 };  // what a pack / unpack moves
+
+// After k_shard_info: the ranges above, and the alignment headers.  A range longer than its message capacity is cut
+// and flagged (SPH_STATUS_HALO_CAPACITY), never written out of bounds.
+__global__ void k_dfsph_shard_ranges(DevParams P, DevArrays S, int32_t *dx, int align_cap, int sweep_cap) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    const int32_t *sd = S.sd;
+    const int layer = P.gy * P.gz;
+    const int sx0 = sd[SD_SX0], sx1 = sd[SD_SX1], o0 = sd[SD_OWN0], o1 = sd[SD_OWN1];
+    auto start_of_layer = [&](int L) {
+        L = min(max(L, 0), P.gx);
+        int c = L * layer;
+        return c > 0 ? S.cell_end[c - 1] : 0;
+    };
+    int sl1 = start_of_layer(min(sx0 + P.sgw, sx1)), sl1e = start_of_layer(min(sx0 + 1, sx1));
+    int sr0 = start_of_layer(max(sx1 - P.sgw, sx0)), sr1b = start_of_layer(max(sx1 - 1, sx0));
+    int gl0 = start_of_layer(sx0 - P.sgw), gl1b = start_of_layer(sx0 - 1);
+    int gr1 = start_of_layer(sx1 + P.sgw), gr1e = start_of_layer(sx1 + 1);
+    if (!P.has_left) { sl1 = sl1e = o0; gl0 = gl1b = o0; }
+    if (!P.has_right) { sr0 = sr1b = o1; gr1 = gr1e = o1; }
+    uint32_t flags = 0u;
+    if (sl1 - o0 > align_cap) { sl1 = o0 + align_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    if (o1 - sr0 > align_cap) { sr0 = o1 - align_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    if (o0 - gl0 > align_cap) { gl0 = o0 - align_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    if (gr1 - o1 > align_cap) { gr1 = o1 + align_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    sl1e = min(sl1e, sl1); sr1b = max(sr1b, sr0); gl1b = max(gl1b, gl0); gr1e = min(gr1e, gr1);
+    if (sl1e - o0 > sweep_cap) { sl1e = o0 + sweep_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    if (o1 - sr1b > sweep_cap) { sr1b = o1 - sweep_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    if (o0 - gl1b > sweep_cap) { gl1b = o0 - sweep_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    if (gr1e - o1 > sweep_cap) { gr1e = o1 + sweep_cap; flags |= SPH_STATUS_HALO_CAPACITY; }
+    if (flags) atomicOr(S.status, flags);
+    dx[DX_SEND_L0] = o0; dx[DX_SEND_L1] = sl1; dx[DX_SEND_L1E] = sl1e;
+    dx[DX_SEND_R0] = sr0; dx[DX_SEND_R1] = o1; dx[DX_SEND_R1B] = sr1b;
+    dx[DX_GHOST_L0] = gl0; dx[DX_GHOST_L1] = o0; dx[DX_GHOST_L1B] = gl1b;
+    dx[DX_GHOST_R0] = o1; dx[DX_GHOST_R1] = gr1; dx[DX_GHOST_R1E] = gr1e;
+    int32_t *h = dx + DX_HDR_SEND;
+    h[0] = sl1 - o0; h[1] = sl1e - o0; h[2] = sd[SD_STEP]; h[3] = 0;
+    h[4] = o1 - sr0; h[5] = o1 - sr1b; h[6] = sd[SD_STEP]; h[7] = 0;
+}
+
+// Pack what goes to the neighbours (blockIdx.y = side: 0 = to the left, 1 = to the right) into the send staging:
+// DX_ALIGN = the 4 records of the sgw boundary layers in this rank's sorted order, DX_VELD / DX_DFS = one 16-byte word
+// per particle of the outermost owned layer.  ctrl (may be NULL): a sweep behind the converged one has nothing new.
+__global__ void k_dfsph_shard_pack(DevParams P, DevArrays S, const int32_t *dx, int what, const DfsphCtrl *ctrl) {
+    if (ctrl && ctrl->done) return;
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    const int side = blockIdx.y;
+    const int b = side == 0 ? dx[DX_SEND_L0] : (what == DX_ALIGN ? dx[DX_SEND_R0] : dx[DX_SEND_R1B]);
+    const int e = side == 0 ? (what == DX_ALIGN ? dx[DX_SEND_L1] : dx[DX_SEND_L1E]) : dx[DX_SEND_R1];
+    if (s >= e - b) return;
+    const int i = b + s;
+    SPH_EMU_CHECK(s < P.halo_cap && i >= 0 && i < P.n);
+    if (what == DX_ALIGN) {
+        S.stage[side][0][s] = S.posm[i];
+        S.stage[side][1][s] = S.veld[i];
+        S.stage[side][2][s] = S.x0id[i];
+        S.stage[side][3][s] = S.misc[i];
+    } else {
+        S.stage[side][0][s] = what == DX_VELD ? S.veld[i] : S.dfs[i];
+    }
+}
+
+// Land what the neighbours sent on the ghost records (blockIdx.y = side: 0 = from the left, 1 = from the right).
+// DX_ALIGN: rec[side][k] = the 4 arrays received; both ranks classified the same fp32 positions, so the sender's
+// boundary layers and this rank's ghost layers hold the same records with the same per-cell counts and only the order
+// inside a cell differs -- after the overwrite, ghost record begin + k IS the sender's boundary record k (cell_end stays
+// valid).  A count mismatch leaves the ghost range alone and a record of another cell is not written; both set
+// SPH_STATUS_GHOST_ALIGN.
+// DX_VELD / DX_DFS: rec[side][0] = the words of the neighbour's outermost owned layer -> this rank's first ghost layer.
+__global__ void k_dfsph_shard_unpack(DevParams P, DevArrays S, int32_t *dx, int what, const DfsphCtrl *ctrl,
+                                     const float4 *rec00, const float4 *rec01, const float4 *rec02, const float4 *rec03,
+                                     const float4 *rec10, const float4 *rec11, const float4 *rec12, const float4 *rec13) {
+    if (ctrl && ctrl->done) return;
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    const int side = blockIdx.y;
+    if (side == 0 ? !P.has_left : !P.has_right) return;
+    const int b = side == 0 ? (what == DX_ALIGN ? dx[DX_GHOST_L0] : dx[DX_GHOST_L1B]) : dx[DX_GHOST_R0];
+    const int e = side == 0 ? dx[DX_GHOST_L1] : (what == DX_ALIGN ? dx[DX_GHOST_R1] : dx[DX_GHOST_R1E]);
+    const float4 *r0 = side == 0 ? rec00 : rec10;
+    if (what != DX_ALIGN) {
+        if (s >= e - b) return;
+        float4 *dst = what == DX_VELD ? S.veld : S.dfs;
+        dst[b + s] = r0[s];
+        return;
+    }
+    const int32_t *h = dx + DX_HDR_RECV + 4 * side;
+    const int first = side == 0 ? e - dx[DX_GHOST_L1B] : dx[DX_GHOST_R1E] - b;  // records of the first ghost layer
+    if (h[0] != e - b || h[1] != first) {
+        if (s == 0) atomicOr(S.status, SPH_STATUS_GHOST_ALIGN);
+        return;
+    }
+    if (s >= e - b) return;
+    const int g = b + s;
+    SPH_EMU_CHECK(s < P.halo_cap && g >= 0 && g < P.n);
+    const float4 p = r0[s], q = S.posm[g];
+    int ci, cj, ck, di, dj, dk;
+    const int c_new = cell_of(P, p.x, p.y, p.z, ci, cj, ck), c_old = cell_of(P, q.x, q.y, q.z, di, dj, dk);
+    if (c_new != c_old) { atomicOr(S.status, SPH_STATUS_GHOST_ALIGN); return; }
+    float4 m = side == 0 ? rec03[s] : rec13[s];
+    m.z = __uint_as_float(__float_as_uint(m.z) | FLAG_GHOST);
+    S.posm[g] = p;
+    S.veld[g] = side == 0 ? rec01[s] : rec11[s];
+    S.x0id[g] = side == 0 ? rec02[s] : rec12[s];
+    S.misc[g] = m;
 }

@@ -572,6 +572,7 @@ __global__ void k_advect(DevParams P, DevArrays S) {
 __global__ void k_enforce_boundary(DevParams P, DevArrays S, int particle_type) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.n) return;
+    if (P.slab_on && (i < S.sd[SD_OWN0] || i >= S.sd[SD_OWN1])) return;  // sharded DFSPH: owned particles only
     uint32_t fl = __float_as_uint(S.misc[i].z);
     int mat = (fl & FLAG_FLUID) ? SPH_MATERIAL_FLUID : SPH_MATERIAL_SOLID;
     if (mat != particle_type || !(fl & FLAG_DYNAMIC)) return;

@@ -176,6 +176,11 @@ def armadillo_bath_dynamic_dfsph():
     return _as_dfsph(armadillo_bath_dynamic())
 
 
+def box_4m_dfsph():
+    """box_4m with the DFSPH solver (dt = 4e-3): the sharded DFSPH workload of bench.py --gpus N."""
+    return _as_dfsph(box_4m())
+
+
 NAMED_SCENES = {
     "dragon_bath": dragon_bath,
     "armadillo_bath_dynamic": armadillo_bath_dynamic,
@@ -187,6 +192,7 @@ NAMED_SCENES = {
     "cube_8k": cube_8k,
     "box_4m": box_4m,
     "box_16m": box_16m,
+    "box_4m_dfsph": box_4m_dfsph,
 }
 
 

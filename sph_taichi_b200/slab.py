@@ -1,4 +1,4 @@
-"""x-slab sharding of one WCSPH scene across the GPUs of a node (one process per GPU).
+"""x-slab sharding of one WCSPH or DFSPH scene across the GPUs of a node (one process per GPU).
 
 The reference is single-device; this is the multi-GPU extension BASELINE.json asks for (SURVEY.md section 8e).
 
@@ -14,6 +14,11 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
   ``SPH_SHARD_GRAPH=1``).  The host (this module) only builds the scene, hands the library its share and launches
   steps; it never waits on the device inside a step.  Cuts are re-balanced on the device every
   ``rebalance_every`` steps.
+* DFSPH scenes (``simulationMethod: 4``) step through ``sph_shard_dfsph_step``: the same sort, re-balancing and
+  record exchange, plus a once-per-step ghost alignment and two small exchanges of the outermost owned layer per
+  Jacobi sweep; the loops' error sums are all-gathered and added in rank order, so every rank runs the same sweeps.
+  That step waits on the host once per batch of sweeps, like the single-GPU DFSPH step, and is always launched
+  eagerly: ``SPH_SHARD_GRAPH`` does not apply to it.
 
 ``tests/test_slab_gloo.py`` runs the same library code on the CPU: the host-emulated build of the kernels
 (tests/emu/) with ``GlooTransport`` -- torch.distributed point-to-point over gloo -- in place of NCCL.
@@ -37,6 +42,7 @@ RECORD_ARRAYS = 4  # posm, veld, x0id, misc (acc is recomputed every step and no
 INFO_KEYS = ("n_live", "owned", "x_lo", "x_hi", "step", "own_begin", "own_end", "sendL_begin", "sendL_end",
              "sendR_begin", "sendR_end", "recv_left", "recv_right", "n_sorted", "status")
 STATUS_OUT_OF_GRID, STATUS_HALO_CAPACITY, STATUS_SHARD_CAPACITY = 1, 4, 8
+STATUS_SHARD_VELOCITY, STATUS_GHOST_ALIGN = 16, 32  # sharded DFSPH (include/sph_b200.h)
 
 
 def plan_slabs(layer_counts, world, min_width=SEND_LAYERS + 1):
@@ -117,9 +123,12 @@ class ShardedSimulation:
     """This rank's share of a sharded scene: a CUDA engine in slab mode + the library's halo exchange."""
 
     def __init__(self, cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, uniform_hint, group=None,
-                 rebalance_every=8, transport=None):
+                 rebalance_every=8, transport=None, n_fluid=None):
         from . import engine as _engine
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
+        self.dfsph = cfg.get_cfg("simulationMethod") == 4
+        if self.dfsph and not n_fluid:
+            raise ValueError("a sharded DFSPH scene needs n_fluid, the fluid particle count of ALL ranks")
         self.device = torch.device(device)
         self.slabs0 = [tuple(int(v) for v in s_) for s_ in slabs]
         ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
@@ -133,6 +142,17 @@ class ShardedSimulation:
         self.eng = _engine.Engine(params, n_max=self.n_cap, n_solid=0, n_bodies=0, device=self.device)
         e = self.eng
         self._load(mine, n_mine, uniform_hint)
+        self.last_iterations_v = self.last_iterations = 0
+        self._io = None
+        if self.dfsph:
+            e.set_dfsph(True)
+            # the constants of DFSPHSolver (DFSPH.py:10-17) and its step(): eta, eta_v and the multiply_time_step factors
+            dt, rho0 = float(cfg.get_cfg("timeStepSize")), float(cfg.get_cfg("density0"))
+            max_error_v, max_error = 0.1, 0.05
+            self._io = _lib.SphDfsphStep(enable_divergence_solver=1, max_iterations_v=100, max_iterations=100,
+                                         eta_v=1.0 / dt * max_error_v * 0.01 * rho0, eta=max_error * 0.01 * rho0,
+                                         inv_dt=1 / dt, dt=dt, inv_dt2=1 / (dt * dt), density0=rho0,
+                                         n_fluid=int(n_fluid), first_batch_v=2, first_batch=3)
         # ---- transport: NCCL inside the library (its own communicator), or a caller-supplied one (tests) ----
         if transport is not None:
             self._transport = transport
@@ -179,12 +199,28 @@ class ShardedSimulation:
 
     # ---- stepping --------------------------------------------------------------------------------------
     def step(self, n=1):
+        """``n`` sharded steps.  DFSPH: ``last_iterations_v`` / ``last_iterations`` (and ``last_avg_err_v`` /
+        ``last_avg_err``) are those of the last step, the same on every rank; the call waits on the device once per
+        batch of Jacobi sweeps."""
         e = self.eng
-        e._check(e.lib.sph_shard_step(e.ctx, int(n), e._stream()), "sph_shard_step")
+        if self.dfsph:
+            io = self._io
+            e._check(e.lib.sph_shard_dfsph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_dfsph_step")
+            self.last_iterations_v, self.last_iterations = int(io.iterations_v), int(io.iterations)
+            self.last_avg_err_v, self.last_avg_err = float(io.avg_err_v), float(io.avg_err)
+        else:
+            e._check(e.lib.sph_shard_step(e.ctx, int(n), e._stream()), "sph_shard_step")
         self.steps_done += int(n)
 
+    def transport_stats(self):
+        """(transport groups issued, bytes this rank sent in them) since the engine was created."""
+        out = (C.c_uint64 * 2)()
+        e = self.eng
+        e._check(e.lib.sph_shard_transport_stats(e.ctx, out), "sph_shard_transport_stats")
+        return int(out[0]), int(out[1])
+
     def profile_step(self):
-        """ONE un-graphed step with CUDA events between the stages (synchronises)."""
+        """ONE un-graphed step with CUDA events between the stages (synchronises; WCSPH only)."""
         e = self.eng
         buf = (C.c_float * 6)()
         e._check(e.lib.sph_shard_profile_step(e.ctx, buf, e._stream()), "sph_shard_profile_step")
@@ -206,6 +242,12 @@ class ShardedSimulation:
         if st & (STATUS_HALO_CAPACITY | STATUS_SHARD_CAPACITY):
             raise RuntimeError(f"rank {self.rank}: slab capacity exceeded (status {st}: halo_capacity {self.halo_cap}, "
                                f"capacity {self.n_cap}, live {d['n_live']}); raise capacity_factor")
+        if st & STATUS_SHARD_VELOCITY:
+            raise RuntimeError(f"rank {self.rank}: a particle moved a whole cell layer in x within one step "
+                               f"(|v_x| * dt >= h); the record exchange may have lost it -- reduce timeStepSize")
+        if st & STATUS_GHOST_ALIGN:
+            raise RuntimeError(f"rank {self.rank}: a neighbour's boundary layers and this rank's ghost layers differ "
+                               f"(status {st})")
         return d
 
     @property
@@ -283,7 +325,7 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     ghost_est = 2 * GHOST_LAYERS * int(hist.max())
     n_cap = int((n_mine + ghost_est) * capacity_factor) + 4 * halo_cap + 1024  # live + trash + 2 receive regions
     sim = ShardedSimulation(cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, hint, group=group,
-                            rebalance_every=rebalance_every, transport=transport)
+                            rebalance_every=rebalance_every, transport=transport, n_fluid=int(fluid.sum()))
     return sim, counts["total"]
 
 
@@ -361,17 +403,34 @@ def bench_main(args):
 
     # ---- parity_check + the same-run single-GPU time: rank 0 steps the SAME scene on one GPU ----
     P = int(os.environ.get("SPH_BENCH_PARITY_STEPS", "20"))
-    sim.step(P)
+    counts_sharded = []
+    if sim.dfsph:  # one step per call: the Jacobi iteration counts of every step
+        for _ in range(P):
+            sim.step(1)
+            counts_sharded.append([sim.last_iterations_v, sim.last_iterations])
+    else:
+        sim.step(P)
     gathered = gather_owned(sim)
     parity, strong = None, None
     if rank == 0:
         ps = ParticleSystem(SimConfig(sc), device=dev)
         solver = ps.build_solver()
         solver.initialize()
-        solver.step(P)
+        counts_single = []
+        if sim.dfsph:
+            for _ in range(P):
+                solver.step(1)
+                counts_single.append([solver.last_iterations_v, solver.last_iterations])
+        else:
+            solver.step(P)
         parity = dict(compare_with_single(gathered, ps, d), steps=P, against="the single-GPU engine on rank 0, same scene, "
                       "particles matched by x_0")
         parity["ok"] = bool(parity["same_particle_set"] and parity["max_dx_over_d"] < 1e-3)
+        if sim.dfsph:
+            # the rule of test_dfsph_steps_vs_oracle: tight when both ran the same sweeps
+            same = counts_sharded == counts_single
+            parity.update(iterations_sharded=counts_sharded, iterations_single=counts_single, counts_match=same)
+            parity["ok"] = bool(parity["same_particle_set"] and parity["max_dx_over_d"] < (2e-3 if same else 5e-2))
         K1 = max(3, min(K, 20))
         solver.step(3)
         torch.cuda.synchronize()
@@ -400,15 +459,22 @@ def bench_main(args):
     torch.cuda.synchronize()
     if sampler:
         sampler.start()
-    info0, launches0 = sim.info(), sim.launch_count()
+    info0, launches0, xfer0 = sim.info(), sim.launch_count(), sim.transport_stats()
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     dist.barrier()
     torch.cuda.synchronize()
+    iters = []
     a.record()
-    sim.step(K)
+    if sim.dfsph:
+        for _ in range(K):
+            sim.step(1)
+            iters.append([sim.last_iterations_v, sim.last_iterations])
+    else:
+        sim.step(K)
     b.record()
     torch.cuda.synchronize()
     dist.barrier()
+    xfer1 = sim.transport_stats()
     ms = torch.tensor([a.elapsed_time(b)], device=dev)
     dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     info1 = sim.info()
@@ -421,6 +487,12 @@ def bench_main(args):
     clocks = sampler.stop() if sampler else None
     slabs = [None] * world
     dist.all_gather_object(slabs, [info1["x_lo"], info1["x_hi"]])
+
+    xfer = torch.tensor([float(xfer1[0] - xfer0[0]), float(xfer1[1] - xfer0[1])], device=dev, dtype=torch.float64)
+    dist.all_reduce(xfer, op=dist.ReduceOp.SUM)
+    if sim.dfsph:
+        return _bench_dfsph_tail(args, sim, rank, world, local, name, sc, n_total, parity, strong, ms, tot, mx, clocks,
+                                 iters, xfer)
 
     # ---- per-kernel times on every rank: CUDA events between the stages of un-graphed steps ----
     acc = {}
@@ -520,6 +592,59 @@ def bench_main(args):
                                       "exchange_on_comm_stream": float(roof_max[5].item())},
             "cpu_baseline": None,
             "notes": "cpu_baseline is reported by the N = 1 run and by --impl reference (bench.py contract)",
+        }
+        print(json.dumps(line))
+    dist.barrier()
+    dist.destroy_process_group()
+    return 0
+
+
+def _gpu_name_and_power_limit(index):
+    """(card name, enforced power limit in W) of GPU `index`, read now (nvidia-smi query; None if unavailable)."""
+    import subprocess
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i",
+                              str(index)], capture_output=True, text=True, timeout=20).stdout.strip().split(",")
+        return out[0].strip(), float(out[1])
+    except Exception:  # noqa: BLE001 - informational only
+        return None, None
+
+
+def _bench_dfsph_tail(args, sim, rank, world, local, name, sc, n_total, parity, strong, ms, tot, mx, clocks, iters,
+                      xfer):
+    """The bench line of a sharded DFSPH run.  The WCSPH stage profile (sph_shard_profile_step) does not apply; the
+    line reports the Jacobi iteration counts of the timed steps and the transport traffic instead."""
+    import bench as _bench
+    K, W = args.steps, args.warmup
+    card, plimit = _gpu_name_and_power_limit(local)
+    if rank == 0:
+        t_ms = float(ms.item())
+        val = K / (t_ms * 1e-3)
+        strong.update(tN_ms=t_ms / K, speedup=strong["t1_ms"] / (t_ms / K), n_gpus=world)
+        sweeps = [iv + ip for iv, ip in iters]
+        line = {
+            "metric": _bench.METRIC, "value": val * n_total / 1e6, "unit": _bench.UNIT, "steps_per_s": val,
+            "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": t_ms / K, "higher_is_better": True,
+            "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
+            "config": _bench.workload_config(name, sc, n_total, n_total),
+            "gpu": {"name": card, "power_limit_w": plimit, "read": "nvidia-smi on rank 0, same run"},
+            "sharding": {"owned_total": int(tot[0].item()), "owned_max_per_rank": int(mx[0].item()),
+                         "ghost_layers": GHOST_LAYERS, "halo_capacity_records": sim.halo_cap,
+                         "exchange": "DFSPH: per step one ghost alignment, one record exchange, the exchanges that open "
+                                     "the loops and two per Jacobi sweep (NCCL point-to-point issued by libsph_b200.so "
+                                     "on the compute stream, not overlapped); eager launches, one host wait per batch "
+                                     "of sweeps; cuts re-balanced on the device every 8 steps"},
+            "parity_check": parity,
+            "strong_scaling": strong,
+            "dfsph": {"iterations_per_step": iters, "mean_iterations_per_step": sum(sweeps) / max(len(sweeps), 1),
+                      "transport_groups_per_step_all_ranks": float(xfer[0].item()) / K,
+                      "transport_bytes_per_step_all_ranks": float(xfer[1].item()) / K},
+            "halo": {"record_bytes_per_step_all_ranks": float(tot[1].item()) / K,
+                     "note": "records of the end-of-step exchange (64 B each); the transport bytes above count the "
+                             "fixed-size messages actually sent, including the per-sweep ones"},
+            "clocks": clocks,
+            "gpu_launches": int(tot[2].item()),
+            "notes": "iterations_per_step = [divergence, pressure] Jacobi iterations of every timed step",
         }
         print(json.dumps(line))
     dist.barrier()
