@@ -209,7 +209,14 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
  * and the host only launches.  Every record is classified as owned / ghost / dropped from its position
  * alone (both ranks evaluate the same fp32 expression), so migration needs no extra message; cuts move by at
  * most one layer every `rebalance_every` steps, decided identically on both sides of a cut from the owned
- * counts in the headers.  Fluid-only scenes with one fluid (uniform masses); rigid bodies are single-GPU.
+ * counts in the headers.  Scenes with one fluid (uniform masses) and any number of STATIC solids: a solid record
+ * rides the exchange like a fluid one (posm.w = its boundary volume m_V, misc = material, flags, solid_id) and is
+ * staged unchanged, so the caller must pack every solid with its final start-up m_V -- the value the single engine's
+ * sph_boundary_volume computes over the WHOLE scene (a solid's neighbours may sit across a cut).  Dynamic solids
+ * (shape-matched bodies, advected rigid blocks) are single-GPU: sph_shard_configure refuses them, and on a sharded
+ * context sph_set_solid_count refuses the dynamic flag, sph_set_rigid_bodies a body table, and sph_boundary_volume,
+ * sph_compute_com, sph_compute_rigid_rest_cm and sph_solve_constraints refuse to run (they walk solid ids through a
+ * slot map that migration leaves stale for solids of other ranks).
  *
  * DFSPH contexts (sph_set_dfsph(1) before sph_shard_configure) step with sph_shard_dfsph_step instead: the same
  * classification, sort, re-balancing and end-of-step record exchange, plus a once-per-step ghost alignment (each
@@ -243,8 +250,8 @@ int sph_shard_begin(SphCtx *ctx, void *stream);
 /* nsteps sharded SPHBase.step()s (sph_base.py:263-271): asynchronous launches that run ahead of the device (no host
  * synchronisation inside a step); SPH_SHARD_GRAPH=1 replays one captured CUDA graph per step instead */
 int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream);
-/* nsteps sharded DFSPH SPHBase.step()s (sph_base.py:263-271 with DFSPH.substep, DFSPH.py:399-408) of a fluid-only
- * DFSPH context: the step of sph_dfsph_step with `io` used the same way, except that io->n_fluid is the GLOBAL fluid
+/* nsteps sharded DFSPH SPHBase.step()s (sph_base.py:263-271 with DFSPH.substep, DFSPH.py:399-408) of a DFSPH context
+ * (fluid + static solids): the step of sph_dfsph_step with `io` used the same way, except that io->n_fluid is the GLOBAL fluid
  * count (all ranks).  Every rank returns the same iterations, first_batch and avg_err values.  Eager launches with
  * one host wait per batch of Jacobi sweeps, like sph_dfsph_step (SPH_SHARD_GRAPH does not apply).  A particle that
  * moves a whole cell layer in x in one step sets SPH_STATUS_SHARD_VELOCITY (the record exchange would lose it);

@@ -20,6 +20,13 @@ namespace {
 
 std::string g_create_error;
 
+// Sharded contexts hold static solids only.  The solid-id slot map of a rank is not reset or validated under
+// migration (a trash-bucket record may share its id with a live one, a solid on another rank leaves its slot stale),
+// so every entry point that walks it -- boundary volumes, advect-solids, the rigid-body calls -- is refused there.
+const char *const kShardStaticOnly =
+    "x-slab sharding supports static solids only: dynamic solids (shape-matched bodies, advected rigid blocks) and "
+    "the rigid-body and boundary-volume calls that walk solid ids are single-GPU in WCSPH and DFSPH";
+
 constexpr int NUM_TIMERS = 12;
 constexpr int GRAPH_UNROLL = 4;  // must be even (ping-pong parity returns to its start)
 const char *kTimerNames[NUM_TIMERS] = {"zero",  "hash",    "scan",  "bucket",    "rank_move", "boundary_volume",
@@ -496,6 +503,7 @@ int sph_pack(SphCtx *ctx, const SphFields *f, int64_t n, void *stream) {
 int sph_set_solid_count(SphCtx *ctx, int64_t n_solid, int32_t has_dynamic_solids) {
     if (!ctx) return SPH_E_ARG;
     if (n_solid < 0 || n_solid > ctx->n_solid_cap) return fail(ctx, SPH_E_CAPACITY, "n_solid exceeds the capacity given at creation");
+    if (ctx->P.slab_on && n_solid > 0 && has_dynamic_solids) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
     ctx->P.n_solid = (int32_t)n_solid;
     ctx->has_dynamic_solids = has_dynamic_solids != 0;
     drop_graphs(ctx);
@@ -559,6 +567,7 @@ int sph_neighbor_build(SphCtx *ctx, void *stream) {
                                       "(the reference's kernels would read an outdated grid here)");
 
 int sph_boundary_volume(SphCtx *ctx, int32_t moving, void *stream) {
+    if (ctx && ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
     REQUIRE_BUILT(ctx);
     return launch_boundary_volume(ctx, moving, static_cast<cudaStream_t>(stream), &ctx->launches);
 }
@@ -612,6 +621,7 @@ int sph_enforce_boundary(SphCtx *ctx, int32_t particle_type, void *stream) {
 int sph_set_rigid_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodies) {
     if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
     if (n_bodies > ctx->body_cap) return fail(ctx, SPH_E_CAPACITY, "more rigid bodies than the workspace was sized for");
+    if (ctx->P.slab_on && n_bodies > 0) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
     for (int b = 0; b < n_bodies; ++b)  // validate everything before any state changes
         if (bodies[b].solid_begin < 0 || bodies[b].solid_end < bodies[b].solid_begin || bodies[b].solid_end > ctx->n_solid_cap)
             return fail(ctx, SPH_E_ARG, "rigid body solid-id range out of bounds");
@@ -632,6 +642,7 @@ int sph_set_rigid_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodi
 
 static int rigid_call(SphCtx *ctx, int32_t body, int mode, float *out, void *stream) {
     if (!ctx) return SPH_E_ARG;
+    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
     if (body < 0 || body >= (int)ctx->bodies.size()) return fail(ctx, SPH_E_ARG, "rigid body index out of range");
     k_rigid<<<1, RIGID_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S, dev_bodies(ctx), body, mode, out, 0);
     ctx->launches += 1;
@@ -908,8 +919,10 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
     if (!ctx) return SPH_E_ARG;
     if (x_lo < 0 || x_hi > ctx->P.gx || ghost_layers < 1 || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
-    if (!ctx->bodies.empty() || ctx->P.n_solid > 0)
-        return fail(ctx, SPH_E_ARG, "x-slab sharding supports fluid-only scenes (rigid bodies are single-GPU, SURVEY 8e)");
+    // Static solids travel in the records like fluid particles and never change; dynamic solids would need moving
+    // boundary volumes one ghost layer deeper, reactions across a cut and a per-body reduction across ranks.
+    if (!ctx->bodies.empty() || (ctx->P.n_solid > 0 && ctx->has_dynamic_solids))
+        return fail(ctx, SPH_E_ARG, kShardStaticOnly);
     if (!ctx->P.uniform_fluid)
         return fail(ctx, SPH_E_ARG, "x-slab sharding needs a single fluid density (uniform fluid masses)");
     if (halo_capacity < 1 || 2 * halo_capacity + ctx->P.n > ctx->n_max)
@@ -1220,7 +1233,7 @@ int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, 
     return SPH_OK;
 }
 
-// One sharded DFSPH SPHBase.step() (fluid only; no overlap of the exchanges with computation):
+// One sharded DFSPH SPHBase.step() (fluid + static solids; no overlap of the exchanges with computation):
 //   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> densities (owned + first ghost layer) -> factor
 //   -> [density change -> * 1/dt -> dfs exchange -> divergence loop -> * dt] -> non-pressure forces -> predict velocity
 //   -> veld exchange -> density_adv -> * 1/dt^2 -> dfs exchange -> pressure loop -> advect + clamp (owned)

@@ -1180,6 +1180,23 @@ __device__ __forceinline__ void force_pair_packed(const DevParams &P, const DevA
 // (k_shard_info), 2 = only the others, 0 = all -- the halo exchange of the NEXT step starts as soon as the
 // boundary particles are final and overlaps the interior.
 static_assert(LIST_PAD % FORCE_BATCH == 0 && NBR_CAP % LIST_PAD == 0, "list padding must cover a force batch");
+
+// Sharded boundary pass: the record of owned particle i, as it leaves this step, into the send staging of every side
+// whose send range holds i -- slot (0, i - l0) / (1, i - r0), the slot k_shard_apply copies back from.
+__device__ __forceinline__ void shard_stage_record(const DevParams &P, const DevArrays &S, int i, const float4 &p,
+                                                   const float4 &v, const float4 &xo, const float4 &mi) {
+    const int32_t *sd = S.sd;
+#pragma unroll
+    for (int side = 0; side < 2; ++side) {
+        const int b0 = side == 0 ? sd[SD_SEND_L0] : sd[SD_SEND_R0], b1 = side == 0 ? sd[SD_SEND_L1] : sd[SD_SEND_R1];
+        if (i >= b0 && i < b1) {
+            const int slot = i - b0;
+            SPH_EMU_CHECK(slot < P.halo_cap);
+            S.stage[side][0][slot] = p; S.stage[side][1][slot] = v; S.stage[side][2][slot] = xo; S.stage[side][3][slot] = mi;
+        }
+    }
+}
+
 // SHARD: the sharded steps' instantiation (send-range split, staging of the boundary particles); compile-time so
 // that the single-GPU kernel keeps its register budget.
 template <int B, int THREADS, bool FUSE_ADVECT, bool SHARD = false>
@@ -1189,7 +1206,12 @@ __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevP
     auto one = [&](const int i) {
     float4 mi = S.misc[i];
     uint32_t fl = __float_as_uint(mi.z);
-    if (!(fl & FLAG_FLUID)) return;
+    if (!(fl & FLAG_FLUID)) {
+        // a solid of a send range is staged too, unchanged: k_shard_apply copies the staging back over EVERY record
+        // of the send ranges, and the neighbour's ghost copy comes from it (sharded scenes hold static solids only)
+        if (SHARD && FUSE_ADVECT && split_mode == 1) shard_stage_record(P, S, i, S.posm[i], S.veld[i], S.x0id[i], mi);
+        return;
+    }
     if (fl & FLAG_GHOST) return;
     float4 pi, vi;
     ldg256(S.fpv + 2 * (size_t)i, pi, vi);
@@ -1252,17 +1274,7 @@ __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevP
             // sharded boundary pass: the interior DENSITIES are still to come and read the positions of these
             // particles, so the advanced state goes to the send staging only (this IS the pack step; the halo
             // exchange starts right after this kernel) and k_shard_apply copies it back later
-            const int32_t *sd = S.sd;
-            const float4 xo = S.x0id[i];
-#pragma unroll
-            for (int side = 0; side < 2; ++side) {
-                const int b0 = side == 0 ? sd[SD_SEND_L0] : sd[SD_SEND_R0], b1 = side == 0 ? sd[SD_SEND_L1] : sd[SD_SEND_R1];
-                if (i >= b0 && i < b1) {
-                    const int slot = i - b0;
-                    SPH_EMU_CHECK(slot < P.halo_cap);
-                    S.stage[side][0][slot] = p; S.stage[side][1][slot] = v; S.stage[side][2][slot] = xo; S.stage[side][3][slot] = mi;
-                }
-            }
+            shard_stage_record(P, S, i, p, v, S.x0id[i], mi);
         } else if (fl & FLAG_DYNAMIC) {
             S.posm[i] = p;
             S.veld[i] = v;

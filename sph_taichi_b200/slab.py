@@ -19,6 +19,10 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
   Jacobi sweep; the loops' error sums are all-gathered and added in rank order, so every rank runs the same sweeps.
   That step waits on the host once per batch of sweeps, like the single-GPU DFSPH step, and is always launched
   eagerly: ``SPH_SHARD_GRAPH`` does not apply to it.
+* Static solids (``RigidBlocks`` / ``RigidBodies`` with ``isDynamic: false``) ride the record exchange like fluid
+  particles and never change.  Their boundary volumes depend on solid neighbours that may sit across a cut, so
+  ``build_sharded`` computes them once, before the first exchange, over the whole scene exactly as the single engine
+  does (``startup_boundary_volumes``).  Dynamic solids are refused (``STATIC_SOLIDS_ONLY``).
 
 ``tests/test_slab_gloo.py`` runs the same library code on the CPU: the host-emulated build of the kernels
 (tests/emu/) with ``GlooTransport`` -- torch.distributed point-to-point over gloo -- in place of NCCL.
@@ -43,6 +47,79 @@ INFO_KEYS = ("n_live", "owned", "x_lo", "x_hi", "step", "own_begin", "own_end", 
              "sendR_begin", "sendR_end", "recv_left", "recv_right", "n_sorted", "status")
 STATUS_OUT_OF_GRID, STATUS_HALO_CAPACITY, STATUS_SHARD_CAPACITY = 1, 4, 8
 STATUS_SHARD_VELOCITY, STATUS_GHOST_ALIGN = 16, 32  # sharded DFSPH (include/sph_b200.h)
+FLAG_FLUID, FLAG_DYNAMIC, FLAG_GHOST = 1, 2, 4  # misc.z bits of a packed record (csrc/sph_common.cuh)
+STATIC_SOLIDS_ONLY = ("x-slab sharding supports static solids only: dynamic solids (shape-matched bodies, advected "
+                      "rigid blocks) are single-GPU in WCSPH and DFSPH")
+
+
+def scene_params(cfg):
+    """The engine constants of a scene, as ``ParticleSystem`` derives them before a solver overrides any."""
+    from . import engine as _engine
+    ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
+    radius = cfg.get_cfg("particleRadius")
+    grid_num = np.ceil(ds / (radius * 4.0)).astype(int)
+    return _engine.make_params(3, grid_num, radius, cfg.get_cfg("density0"), cfg.get_cfg("stiffness"),
+                               cfg.get_cfg("exponent"), cfg.get_cfg("timeStepSize"), cfg.get_cfg("gravitation"), ds)
+
+
+def solid_ids(arrays):
+    """Global solid ids as ``ParticleSystem._prepare_solids`` assigns them: dense, every object's solids contiguous
+    (stable order by object id), -1 for fluid particles."""
+    solid = np.nonzero(np.asarray(arrays["material"]) == 0)[0]
+    sid = np.full(len(arrays["material"]), -1, np.int32)
+    order = np.argsort(np.asarray(arrays["object_id"])[solid], kind="stable")
+    sid[solid[order]] = np.arange(solid.size, dtype=np.int32)
+    return sid
+
+
+def field_tensors(arrays, n, m_V0, device):
+    """The engine's pack fields of ``n`` particles in the reference's layout (``ParticleSystem.add_particles``:
+    x_0 = x, m = density * m_V0); ``arrays["m_V"]`` / ``arrays["solid_id"]`` are used when present."""
+    def t(a, dt):
+        return torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(device)
+
+    dens = t(arrays["density"], np.float32)
+    m_V = t(arrays["m_V"], np.float32) if "m_V" in arrays else torch.full((n,), m_V0, dtype=torch.float32, device=device)
+    return {
+        "object_id": t(arrays["object_id"], np.int32), "x": t(arrays["x"], np.float32),
+        "x_0": t(arrays["x"], np.float32), "v": t(arrays["v"], np.float32),
+        "acceleration": torch.zeros((n, 3), dtype=torch.float32, device=device),
+        "m_V": m_V, "m": dens * m_V0,
+        "density": dens, "pressure": t(arrays["pressure"], np.float32), "material": t(arrays["material"], np.int32),
+        "is_dynamic": t(arrays["is_dynamic"], np.int32), "color": t(arrays["color"], np.int32),
+        "grid_ids": None, "solid_id": t(arrays["solid_id"], np.int32) if "solid_id" in arrays else None,
+    }
+
+
+def startup_boundary_volumes(cfg, arrays, device):
+    """m_V of every particle of the whole scene after ``SPHBase.initialize()``: the single engine's start-up boundary
+    volumes (``compute_static_boundary_volume`` then ``compute_moving_boundary_volume``), computed by the same kernels
+    on the same packed scene, hence bit-identical to them; fluid particles keep m_V0.  ``arrays`` must hold
+    ``solid_id``.  Every rank runs this on the whole scene, so every rank holds the same value for every solid."""
+    from . import engine as _engine
+    n = len(arrays["material"])
+    sid = np.asarray(arrays["solid_id"])
+    n_solid = int((sid >= 0).sum())
+    m_V0 = float(np.float32(0.8 * (2 * cfg.get_cfg("particleRadius")) ** 3))
+    out = np.full(n, np.float32(m_V0), np.float32)
+    if n_solid == 0:
+        return out
+    eng = _engine.Engine(scene_params(cfg), n_max=n, n_solid=n_solid, n_bodies=0, device=device)
+    try:
+        f = field_tensors(arrays, n, m_V0, device)
+        eng.pack(f, n, n_solid, bool((np.asarray(arrays["is_dynamic"])[sid >= 0] != 0).any()))
+        eng.neighbor_build()
+        eng.boundary_volume(0)
+        eng.boundary_volume(1)
+        eng.unpack(f)  # sorted order; solid_id maps it back
+        got_sid, got_mV = f["solid_id"].cpu().numpy(), f["m_V"].cpu().numpy()
+    finally:
+        eng.close()
+    by_sid = np.empty(n_solid, np.float32)
+    s = got_sid >= 0
+    by_sid[got_sid[s]] = got_mV[s]
+    out[sid >= 0] = by_sid[sid[sid >= 0]]
+    return out
 
 
 def plan_slabs(layer_counts, world, min_width=SEND_LAYERS + 1):
@@ -123,7 +200,10 @@ class ShardedSimulation:
     """This rank's share of a sharded scene: a CUDA engine in slab mode + the library's halo exchange."""
 
     def __init__(self, cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, uniform_hint, group=None,
-                 rebalance_every=8, transport=None, n_fluid=None):
+                 rebalance_every=8, transport=None, n_fluid=None, n_solid=0):
+        """``mine``: this rank's initial particles (numpy arrays in the reference's field layout); with solids also
+        ``solid_id`` (global ids, ``solid_ids``) and ``m_V`` (start-up boundary volumes, ``startup_boundary_volumes``).
+        ``n_solid``: the solid count of the WHOLE scene (sizes the solid-id slot map)."""
         from . import engine as _engine
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dfsph = cfg.get_cfg("simulationMethod") == 4
@@ -135,11 +215,10 @@ class ShardedSimulation:
         radius = cfg.get_cfg("particleRadius")
         self.h = radius * 4.0
         self.grid_num = np.ceil(ds / self.h).astype(int)
-        params = _engine.make_params(3, self.grid_num, radius, cfg.get_cfg("density0"), cfg.get_cfg("stiffness"),
-                                     cfg.get_cfg("exponent"), cfg.get_cfg("timeStepSize"), cfg.get_cfg("gravitation"), ds)
         self.m_V0 = float(np.float32(0.8 * (2 * radius) ** 3))
-        self.n_cap, self.halo_cap = int(n_cap), int(halo_cap)
-        self.eng = _engine.Engine(params, n_max=self.n_cap, n_solid=0, n_bodies=0, device=self.device)
+        self.n_cap, self.halo_cap, self.n_solid = int(n_cap), int(halo_cap), int(n_solid)
+        self.eng = _engine.Engine(scene_params(cfg), n_max=self.n_cap, n_solid=self.n_solid, n_bodies=0,
+                                  device=self.device)
         e = self.eng
         self._load(mine, n_mine, uniform_hint)
         self.last_iterations_v = self.last_iterations = 0
@@ -177,24 +256,13 @@ class ShardedSimulation:
 
     def _load(self, arrays, n, uniform_hint):
         """Pack this rank's initial particles (numpy arrays in the reference's field layout)."""
-        dev = self.device
-
-        def t(a, dt):
-            return torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
-
-        if int((np.asarray(arrays["material"]) != 1).sum()) != 0:
-            raise NotImplementedError("x-slab sharding supports fluid-only scenes (SURVEY.md section 8e)")
-        dens = t(arrays["density"], np.float32)
-        f = {
-            "object_id": t(arrays["object_id"], np.int32), "x": t(arrays["x"], np.float32),
-            "x_0": t(arrays["x"], np.float32), "v": t(arrays["v"], np.float32),
-            "acceleration": torch.zeros((n, 3), dtype=torch.float32, device=dev),
-            "m_V": torch.full((n,), self.m_V0, dtype=torch.float32, device=dev), "m": dens * self.m_V0,
-            "density": dens, "pressure": t(arrays["pressure"], np.float32), "material": t(arrays["material"], np.int32),
-            "is_dynamic": t(arrays["is_dynamic"], np.int32), "color": t(arrays["color"], np.int32),
-            "grid_ids": None, "solid_id": None,
-        }
-        self.eng.pack(f, n, 0, False, uniform_hint=uniform_hint)
+        solid = np.asarray(arrays["material"]) != 1
+        if bool((solid & (np.asarray(arrays["is_dynamic"]) != 0)).any()):
+            raise NotImplementedError(STATIC_SOLIDS_ONLY)
+        if solid.any() and ("solid_id" not in arrays or "m_V" not in arrays):
+            raise ValueError("solid particles need their global solid_id and start-up m_V (see build_sharded)")
+        f = field_tensors(arrays, n, self.m_V0, self.device)
+        self.eng.pack(f, n, self.n_solid, False, uniform_hint=uniform_hint)
         self.synchronize()  # the temporaries above may be freed now
 
     # ---- stepping --------------------------------------------------------------------------------------
@@ -275,16 +343,19 @@ class ShardedSimulation:
         return views
 
     def owned_tensors(self):
-        """(x, v, x_0) of the owned particles as device tensors [owned, 3]."""
+        """(x, v, x_0, object_id, m_V, flags) of the owned particles as device tensors ([owned, 3] / [owned]); flags
+        holds the record's FLAG_* bits (FLAG_FLUID clear: a solid)."""
         d = self.info()
         v = self.record_views()
         b, e_ = d["own_begin"], d["own_end"]
-        ghost = (v[3][b:e_, 2].contiguous().view(torch.int32) & 4) != 0
-        keep = ~ghost
-        return v[0][b:e_, :3][keep], v[1][b:e_, :3][keep], v[2][b:e_, :3][keep]
+        flags = v[3][b:e_, 2].contiguous().view(torch.int32)
+        keep = (flags & FLAG_GHOST) == 0
+        oid = v[2][b:e_, 3].contiguous().view(torch.int32)
+        return (v[0][b:e_, :3][keep], v[1][b:e_, :3][keep], v[2][b:e_, :3][keep], oid[keep], v[0][b:e_, 3][keep],
+                flags[keep])
 
     def owned_state(self):
-        x, v, x0 = self.owned_tensors()
+        x, v, x0 = self.owned_tensors()[:3]
         return x.cpu().numpy(), v.cpu().numpy(), x0.cpu().numpy()
 
     def launch_count(self):
@@ -312,70 +383,104 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     hist = np.bincount(lay, minlength=gx)[:gx]
     if slabs is None:
         slabs = plan_slabs(hist, world)
+    fluid = arrays["material"] == 1
+    if bool((~fluid & (arrays["is_dynamic"] != 0)).any()):
+        raise NotImplementedError(STATIC_SOLIDS_ONLY)
+    n_solid = int((~fluid).sum())
+    if n_solid:
+        arrays["solid_id"] = solid_ids(arrays)
+        arrays["m_V"] = startup_boundary_volumes(cfg, arrays, device)
     lo, hi = slabs[rank]
     mine, n_mine = select_owned(arrays, h, lo, hi)
-    # one decision for the whole scene (a rank may start empty): all fluid particles share m and m_V?
-    fluid = arrays["material"] == 1
-    dens = arrays["density"][fluid].astype(np.float32)
+    # one decision for the whole scene (a rank may start empty), the single engine's: all FLUID particles share m
+    # and m_V (solids do not count)?
     m_V0 = np.float32(0.8 * (2 * radius) ** 3)
-    uniform = bool(fluid.all() and dens.size and (dens == dens[0]).all())
-    hint = (uniform, float(np.float32(m_V0 * dens[0])) if dens.size else 0.0, float(m_V0))
+    m_fluid = arrays["density"][fluid].astype(np.float32) * m_V0
+    uniform = bool(m_fluid.size and (m_fluid == m_fluid[0]).all())
+    hint = (uniform, float(m_fluid[0]) if m_fluid.size else 0.0, float(m_V0))
     # the fullest layer bounds every layer the front may reach later: SEND_LAYERS of them per side and direction
     halo_cap = int(SEND_LAYERS * int(hist.max()) * capacity_factor) + 1024
     ghost_est = 2 * GHOST_LAYERS * int(hist.max())
     n_cap = int((n_mine + ghost_est) * capacity_factor) + 4 * halo_cap + 1024  # live + trash + 2 receive regions
     sim = ShardedSimulation(cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, hint, group=group,
-                            rebalance_every=rebalance_every, transport=transport, n_fluid=int(fluid.sum()))
+                            rebalance_every=rebalance_every, transport=transport, n_fluid=int(fluid.sum()),
+                            n_solid=n_solid)
     return sim, counts["total"]
 
 
 # -----------------------------------------------------------------------------------------------
 # sharded state against the single-GPU engine (bench.py --gpus N parity_check, tools/check_slab_parity.py)
 # -----------------------------------------------------------------------------------------------
-def _lexsort_rows(x0):
-    """Permutation sorting the rows of a [n, 3] tensor lexicographically (x, then y, then z) on its device."""
+def _lexsort_rows(x0, oid=None):
+    """Permutation sorting the rows of a [n, 3] tensor lexicographically (x, then y, then z) on its device; with
+    ``oid`` the object id is the leading key."""
     order = torch.arange(x0.shape[0], device=x0.device)
     for col in (2, 1, 0):
         _, idx = torch.sort(x0[order, col], stable=True)
+        order = order[idx]
+    if oid is not None:
+        _, idx = torch.sort(oid[order], stable=True)
         order = order[idx]
     return order
 
 
 def gather_owned(sim, dst=0):
-    """All ranks' owned (x, v, x_0) gathered on rank `dst` as device tensors (None elsewhere)."""
-    x, v, x0 = sim.owned_tensors()
-    rec = torch.cat([x, v, x0], dim=1).contiguous()
+    """All ranks' owned (x, v, x_0, object_id, m_V, flags) gathered on rank `dst` as device tensors (None
+    elsewhere)."""
+    x, v, x0, oid, m_V, flags = sim.owned_tensors()
+    rec = torch.cat([x, v, x0, oid.view(torch.float32)[:, None], m_V[:, None], flags.view(torch.float32)[:, None]],
+                    dim=1).contiguous()
+
+    def split(t):
+        return (t[:, 0:3], t[:, 3:6], t[:, 6:9], t[:, 9].contiguous().view(torch.int32), t[:, 10].contiguous(),
+                t[:, 11].contiguous().view(torch.int32))
+
     if sim.world == 1:
-        return rec[:, 0:3], rec[:, 3:6], rec[:, 6:9]
+        return split(rec)
     n = torch.tensor([rec.shape[0]], device=rec.device, dtype=torch.int64)
     counts = [torch.zeros_like(n) for _ in range(sim.world)]
     dist.all_gather(counts, n, group=sim.group)
     counts = [int(c.item()) for c in counts]
     cap = max(counts)
-    pad = torch.zeros((cap, 9), device=rec.device, dtype=rec.dtype)
+    pad = torch.zeros((cap, rec.shape[1]), device=rec.device, dtype=rec.dtype)
     pad[:rec.shape[0]] = rec
     bufs = [torch.empty_like(pad) for _ in range(sim.world)] if sim.rank == dst else None
     dist.gather(pad, bufs, dst=dst, group=sim.group)
     if sim.rank != dst:
         return None
-    full = torch.cat([b[:c] for b, c in zip(bufs, counts)], dim=0)
-    return full[:, 0:3], full[:, 3:6], full[:, 6:9]
+    return split(torch.cat([b[:c] for b, c in zip(bufs, counts)], dim=0))
 
 
 def compare_with_single(gathered, ps, d):
-    """Rank 0: the gathered sharded state against a ParticleSystem that ran the same steps on ONE GPU."""
-    X, V, X0 = gathered
+    """Rank 0: the gathered sharded state against a ParticleSystem that ran the same steps on ONE GPU, particles
+    matched by (object_id, x_0).  With solids in the scene it also reports whether every static solid is still
+    exactly at x_0 and the largest relative difference of the static solids' m_V from the single engine's."""
+    X, V, X0, OID, MV, FL = gathered
     ps._pull()
-    rx, rv, rx0 = ps._t["x"], ps._t["v"], ps._t["x_0"]
+    n = int(ps.particle_num[None])
+    rx, rv, rx0, roid, rmv = (ps._t[k][:n] for k in ("x", "v", "x_0", "object_id", "m_V"))
     same = tuple(X0.shape) == tuple(rx0.shape)
     dx = dv = float("inf")
+    out = {}
     if same:
-        ks, kr = _lexsort_rows(X0), _lexsort_rows(rx0)
-        same = bool(torch.equal(X0[ks], rx0[kr]))
+        ks, kr = _lexsort_rows(X0, OID), _lexsort_rows(rx0, roid)
+        same = bool(torch.equal(X0[ks], rx0[kr]) and torch.equal(OID[ks], roid[kr]))
         if same:
             dx = float((X[ks] - rx[kr]).abs().max().item() / d)
             dv = float((V[ks] - rv[kr]).abs().max().item())
-    return {"same_particle_set": bool(same), "max_dx_over_d": dx, "max_dv": dv, "particles": int(X0.shape[0])}
+            static = ((FL[ks] & (FLAG_FLUID | FLAG_DYNAMIC)) == 0)
+            if bool(static.any()):
+                a, b = MV[ks][static].double(), rmv[kr][static].double()
+                out = {"static_solids": int(static.sum().item()),
+                       "static_solids_at_x0": bool(torch.equal(X[ks][static], X0[ks][static])),
+                       "max_rel_dm_V_static": float(((a - b).abs() / b.abs()).max().item())}
+    return dict({"same_particle_set": bool(same), "max_dx_over_d": dx, "max_dv": dv, "particles": int(X0.shape[0])},
+                **out)
+
+
+def static_solids_ok(cmp_):
+    """The static-solid part of a ``compare_with_single`` result (true without static solids)."""
+    return cmp_.get("static_solids_at_x0", True) and cmp_.get("max_rel_dm_V_static", 0.0) < 1e-6
 
 
 # -----------------------------------------------------------------------------------------------
@@ -424,13 +529,14 @@ def bench_main(args):
         else:
             solver.step(P)
         parity = dict(compare_with_single(gathered, ps, d), steps=P, against="the single-GPU engine on rank 0, same scene, "
-                      "particles matched by x_0")
-        parity["ok"] = bool(parity["same_particle_set"] and parity["max_dx_over_d"] < 1e-3)
+                      "particles matched by (object_id, x_0)")
+        parity["ok"] = bool(parity["same_particle_set"] and parity["max_dx_over_d"] < 1e-3 and static_solids_ok(parity))
         if sim.dfsph:
             # the rule of test_dfsph_steps_vs_oracle: tight when both ran the same sweeps
             same = counts_sharded == counts_single
             parity.update(iterations_sharded=counts_sharded, iterations_single=counts_single, counts_match=same)
-            parity["ok"] = bool(parity["same_particle_set"] and parity["max_dx_over_d"] < (2e-3 if same else 5e-2))
+            parity["ok"] = bool(parity["same_particle_set"] and parity["max_dx_over_d"] < (2e-3 if same else 5e-2)
+                                and static_solids_ok(parity))
         K1 = max(3, min(K, 20))
         solver.step(3)
         torch.cuda.synchronize()

@@ -3,8 +3,11 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         --master-port 29533 tools/check_slab_parity.py --counts 64 24 24 --steps 60
 
-Rank 0 also runs the plain single-GPU engine and compares every particle (matched by x_0).
+Rank 0 also runs the plain single-GPU engine and compares every particle (matched by object_id and x_0).
 Prints one JSON line and exits non-zero on mismatch.
+
+--static-block puts a static rigid block under the fluid, across every cut; the tool then also checks that every
+static solid is still exactly at x_0 with the single engine's start-up boundary volume m_V.
 
 --dfsph runs the scene with the DFSPH solver (dt = 4e-3) and also compares the Jacobi iteration counts of every step
 with the single engine's, checks that every rank reported bit-identical counts and average errors in every step, and
@@ -30,6 +33,20 @@ import torch.distributed as dist
 from sph_taichi_b200 import ParticleSystem, SimConfig, scene, slab
 
 
+def static_block_scene(c, d):
+    """The dam break one spacing above a static floor block (object 1, three lattice layers thick) that spans twice
+    the fluid's x extent and its whole z extent: every cut of the fluid also cuts the block, and the fluid slides
+    along it."""
+    sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12],
+                             start=[0.06, 0.10, 0.06])
+    lo = [0.04, 0.04, 0.04]
+    n = [2 * c[0], 3, c[2] + 2]
+    sc["RigidBlocks"] = [{"objectId": 1, "start": lo, "end": [s + (k - 0.5) * d for s, k in zip(lo, n)],
+                          "translation": [0.0, 0.0, 0.0], "scale": [1, 1, 1], "velocity": [0.0, 0.0, 0.0],
+                          "density": 1000.0, "color": [255, 255, 255], "isDynamic": False}]
+    return sc
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--counts", type=int, nargs=3, default=[64, 24, 24])
@@ -38,6 +55,11 @@ def main():
     ap.add_argument("--skew", type=int, default=0, help="shift every interior slab cut by this many layers at the start")
     ap.add_argument("--rebalance-every", type=int, default=8)
     ap.add_argument("--dfsph", action="store_true", help="DFSPH instead of WCSPH (simulationMethod 4, dt = 4e-3)")
+    ap.add_argument("--static-block", action="store_true",
+                    help="the fluid rests on a static rigid block that straddles every cut (static_block_scene)")
+    ap.add_argument("--scene", default=None, choices=sorted(scene.NAMED_SCENES),
+                    help="a named scene as it is (--counts, --vx and --static-block do not apply; a DFSPH scene needs "
+                         "--dfsph for the iteration-count comparison)")
     ap.add_argument("--soak", type=int, default=0, metavar="EVERY",
                     help="long run: read the step state (capacity / out-of-grid flags raise) every EVERY steps; the "
                          "flow is chaotic over thousands of steps, so the verdict is the particle set, finiteness and "
@@ -54,9 +76,16 @@ def main():
             dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
     d = 0.02
     c = a.counts
-    sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12], start=[0.06] * 3)
-    sc["FluidBlocks"][0]["velocity"] = [a.vx, 0.0, 0.0]
-    if a.dfsph:
+    if a.scene:
+        sc = scene.NAMED_SCENES[a.scene]()
+        d = 2.0 * sc["Configuration"]["particleRadius"]
+    elif a.static_block:
+        sc = static_block_scene(c, d)
+    else:
+        sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12], start=[0.06] * 3)
+    if not a.scene:
+        sc["FluidBlocks"][0]["velocity"] = [a.vx, 0.0, 0.0]
+    if a.dfsph and sc["Configuration"]["simulationMethod"] != 4:
         sc = scene._as_dfsph(sc)
     transport = slab.GlooTransport() if (EMU and world > 1) else None
     slabs = None
@@ -119,7 +148,11 @@ def main():
         cmp_ = slab.compare_with_single(gathered, ps, d)
         migrated = any(m["owned"][0] != m["owned"][1] for m in metas)
         moved = any(tuple(m["slab0"]) != tuple(m["slab1"]) for m in metas)
-        ok = cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < 1e-3 and cmp_["max_dv"] < 1e-2
+        ok = cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < 1e-3 and cmp_["max_dv"] < 1e-2 and slab.static_solids_ok(cmp_)
+        solid = ps._t["material"][:n_total] == 0
+        if bool(solid.any()):  # [first, last + 1) cell layer the solids occupy
+            lay = slab.layer_of(ps._t["x"][:n_total][solid].cpu().numpy(), 2 * d)
+            cmp_["solid_layers"] = [int(lay.min()), int(lay.max()) + 1]
         if a.dfsph:
             counts = [list(t[:2]) for t in metas[0]["trace"]]
             same_on_ranks = all([list(t) for t in m["trace"]] == [list(t) for t in metas[0]["trace"]] for m in metas)
@@ -132,13 +165,14 @@ def main():
             counts_match = counts == single_counts
             # the rule of test_dfsph_steps_vs_oracle: tight when the solvers ran the same sweeps
             tol = 2e-3 if counts_match else 5e-2
-            ok = cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < tol and same_on_ranks and aligned
+            ok = (cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < tol and same_on_ranks and aligned
+                  and slab.static_solids_ok(cmp_))
             cmp_ = dict(cmp_, iterations_sharded=counts, iterations_single=single_counts, counts_match=counts_match,
                         bit_identical_across_ranks=same_on_ranks, ghosts_aligned=aligned,
                         transport_groups=[m["transport"][0] for m in metas],
                         transport_bytes=[m["transport"][1] for m in metas])
         if a.soak:
-            X, V, _ = gathered
+            X, V = gathered[:2]
             ps._pull()
             rx, rv = ps._t["x"], ps._t["v"]
             bulk = {"com_sharded": [round(float(t), 5) for t in X.double().mean(0)],
