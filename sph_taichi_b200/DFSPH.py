@@ -25,6 +25,25 @@ from .sph_base import SPHBase
 (OP_DENSITIES, OP_FACTOR, OP_DENSITY_CHANGE, OP_DENSITY_ADV, OP_DENSITY_ERROR, OP_MULTIPLY_FACTOR,
  OP_DIVERGENCE_ITERATION, OP_PRESSURE_ITERATION, OP_NON_PRESSURE, OP_PREDICT_VELOCITY, OP_ADVECT) = range(11)
 
+# The reference solver's constants (DFSPH.py:10-17).  The sharded engine (slab.ShardedSimulation) steps with the same
+# ones through dfsph_step_io, so that it matches the single engine it is compared with.
+MAX_ITERATIONS_V = MAX_ITERATIONS = 100
+MAX_ERROR_V, MAX_ERROR = 0.1, 0.05
+FIRST_BATCHES = (2, 3)  # first batch of sweeps of the divergence / pressure solve before a step has counted them
+
+
+def dfsph_step_io(dt, density0, n_fluid, first_batch_v=FIRST_BATCHES[0], first_batch=FIRST_BATCHES[1], *,
+                  enable_divergence_solver=True, max_iterations_v=MAX_ITERATIONS_V, max_iterations=MAX_ITERATIONS,
+                  max_error_v=MAX_ERROR_V, max_error=MAX_ERROR):
+    """The ``SphDfsphStep`` of ``sph_dfsph_step`` / ``sph_shard_dfsph_step``: the loops' limits and thresholds (eta_v,
+    eta as in divergence_solve / pressure_solve) and the multiply_time_step factors of a step of size ``dt``."""
+    from ._lib import SphDfsphStep
+    return SphDfsphStep(enable_divergence_solver=int(bool(enable_divergence_solver)),
+                        max_iterations_v=int(max_iterations_v), max_iterations=int(max_iterations),
+                        eta_v=1.0 / dt * max_error_v * 0.01 * density0, eta=max_error * 0.01 * density0,
+                        inv_dt=1 / dt, dt=dt, inv_dt2=1 / (dt * dt), density0=density0, n_fluid=int(n_fluid),
+                        first_batch_v=first_batch_v, first_batch=first_batch)
+
 
 class DFSPHSolver(SPHBase):
     def __init__(self, particle_system):
@@ -32,16 +51,16 @@ class DFSPHSolver(SPHBase):
         self.surface_tension = 0.01
         self.dt[None] = self.ps.cfg.get_cfg("timeStepSize")
         self.enable_divergence_solver = True
-        self.m_max_iterations_v = 100
-        self.m_max_iterations = 100
+        self.m_max_iterations_v = MAX_ITERATIONS_V
+        self.m_max_iterations = MAX_ITERATIONS
         self.m_eps = 1e-5
-        self.max_error_V = 0.1
-        self.max_error = 0.05
+        self.max_error_V = MAX_ERROR_V
+        self.max_error = MAX_ERROR
         self.verbose = False
         self.device_side_loops = os.environ.get("SPH_DFSPH_HOST_LOOPS", "0") in ("", "0")  # A/B switch
         self.last_iterations_v = 0
         self.last_iterations = 0
-        self._sweeps_guess = [2, 3]  # first batch of the next divergence / pressure solve (updated every step)
+        self._sweeps_guess = list(FIRST_BATCHES)  # first batches of the next two solves (updated every step)
         self.ps._engine.set_dfsph(True)
         self._err = torch.zeros(1, dtype=torch.float64, device=self.ps.device)
 
@@ -154,16 +173,11 @@ class DFSPHSolver(SPHBase):
         """sph_base.py:263-271.  With device-side loops the whole step is one library call."""
         if not self.device_side_loops:
             return super().step(n)
-        from ._lib import SphDfsphStep
         ps = self.ps
-        dt = self.dt[None]
-        io = SphDfsphStep(enable_divergence_solver=int(bool(self.enable_divergence_solver)),
-                          max_iterations_v=int(self.m_max_iterations_v), max_iterations=int(self.m_max_iterations),
-                          eta_v=1.0 / dt * self.max_error_V * 0.01 * self.density_0,
-                          eta=self.max_error * 0.01 * self.density_0,
-                          inv_dt=1 / dt, dt=dt, inv_dt2=1 / (dt * dt), density0=self.density_0,
-                          n_fluid=int(ps.fluid_particle_num), first_batch_v=self._sweeps_guess[0],
-                          first_batch=self._sweeps_guess[1])
+        io = dfsph_step_io(self.dt[None], self.density_0, ps.fluid_particle_num, *self._sweeps_guess,
+                           enable_divergence_solver=self.enable_divergence_solver,
+                           max_iterations_v=self.m_max_iterations_v, max_iterations=self.m_max_iterations,
+                           max_error_v=self.max_error_V, max_error=self.max_error)
         ps._push()
         ps._engine.dfsph_step(n, io)
         ps._after_engine()

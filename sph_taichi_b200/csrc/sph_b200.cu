@@ -76,6 +76,34 @@ Layout make_layout(int64_t n_max, int64_t C, int64_t n_solid, int n_bodies) {
     return L;
 }
 
+constexpr uint64_t SHARD_HDR_BYTES = 64;  // the 16-int header that travels with every record exchange
+
+// The shard buffer (library-owned, x-slab sharding): {device step state | send header x 2 | 2 sides x 4 send staging
+// arrays x halo_cap records | sharded DFSPH: DX ranges + alignment headers | one fp64 error partial per rank}
+struct ShardLayout {
+    uint64_t off_state, off_hdr[2], off_stage[2][4], off_dx, off_err;
+    uint64_t total;
+};
+
+ShardLayout make_shard_layout(int64_t halo_cap, int world) {
+    ShardLayout L;
+    uint64_t o = 0;
+    auto take = [&](uint64_t bytes) { uint64_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.off_state = take(SD_INTS * 4);
+    for (int side = 0; side < 2; ++side) L.off_hdr[side] = take(SHARD_HDR_BYTES);
+    for (int side = 0; side < 2; ++side)
+        for (int k = 0; k < 4; ++k) L.off_stage[side][k] = take((uint64_t)halo_cap * 16);
+    L.off_dx = take(DX_INTS * 4);
+    L.off_err = take((uint64_t)world * 8);
+    L.total = o;
+    return L;
+}
+
+struct GraphSlot {  // one instantiated CUDA graph and the kernels a replay of it launches
+    cudaGraphExec_t exec = nullptr;
+    int64_t kernels = 0;
+};
+
 #ifndef SPH_EMU
 // NCCL point-to-point through dlopen: the library has no link-time dependency on NCCL (the CPU test-suite and
 // single-GPU users never load it); inside a PyTorch process the already loaded libnccl.so.2 is reused.
@@ -133,10 +161,8 @@ struct SphCtx {
     std::string err;
     int64_t launches = 0;
     // CUDA graphs, one per ping-pong parity
-    cudaGraphExec_t graph[2] = {nullptr, nullptr};
-    int64_t graph_kernels[2] = {0, 0};
-    cudaGraphExec_t graph_multi[2] = {nullptr, nullptr};  // GRAPH_UNROLL steps per replay
-    int64_t graph_multi_kernels[2] = {0, 0};
+    GraphSlot graph[2];
+    GraphSlot graph_multi[2];  // GRAPH_UNROLL steps per replay
     int parity = 0;
     int var_density = 1, var_force = 1;  // 1 = production; 0 = ablation variants (SPH_DENSITY_VARIANT / SPH_FORCE_VARIANT)
     bool time_pair = false;
@@ -150,11 +176,11 @@ struct SphCtx {
     int rank = 0, world = 1;
     void *nccl_comm = nullptr;
     char *shard_buf = nullptr;  // library-owned: device step state + send staging (cudaMalloc at sph_shard_configure)
+    ShardLayout SL{};
     bool shard_begun = false;
     cudaStream_t comm_stream = nullptr;
     cudaEvent_t ev_packed = nullptr, ev_exchanged = nullptr;
-    cudaGraphExec_t graph_shard[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [parity][wide exchange]
-    int64_t graph_shard_kernels[2][2] = {{0, 0}, {0, 0}};
+    GraphSlot graph_shard[2][2];  // [parity][wide exchange]
     int32_t narrow_cap = 0;      // records per side of the usual (sgw + 1 layers) exchange; halo_cap = sgw + 2 layers
     // hide the exchange behind the interior densities too (boundary densities first): meant for a rank that talks to
     // two neighbours, whose exchange can outlast the interior force pass; with one neighbour or short exchanges the
@@ -220,12 +246,12 @@ void bind_arrays(SphCtx *c) {
     S.nbr_cnt = reinterpret_cast<int32_t *>(w + L.off_nbr_cnt);
     S.npad = (int32_t)L.npad;
     S.sd = nullptr;
-    if (c->shard_buf) {  // {state ints | header x 2 | 2 sides x 4 arrays x halo_cap records}
-        S.sd = reinterpret_cast<int32_t *>(c->shard_buf);
-        char *q = c->shard_buf + 256;
-        for (int side = 0; side < 2; ++side) { S.stage_hdr[side] = reinterpret_cast<int32_t *>(q); q += 256; }
-        for (int side = 0; side < 2; ++side)
-            for (int k = 0; k < 4; ++k) { S.stage[side][k] = reinterpret_cast<float4 *>(q); q += align_up((uint64_t)c->P.halo_cap * 16, 256); }
+    if (c->shard_buf) {
+        S.sd = reinterpret_cast<int32_t *>(c->shard_buf + c->SL.off_state);
+        for (int side = 0; side < 2; ++side) {
+            S.stage_hdr[side] = reinterpret_cast<int32_t *>(c->shard_buf + c->SL.off_hdr[side]);
+            for (int k = 0; k < 4; ++k) S.stage[side][k] = reinterpret_cast<float4 *>(c->shard_buf + c->SL.off_stage[side][k]);
+        }
     }
 }
 
@@ -261,11 +287,11 @@ inline void pdl_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream
 #endif
 
 void drop_graphs(SphCtx *c) {
+    auto drop = [](GraphSlot &g) { if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; } };
     for (int k = 0; k < 2; ++k) {
-        if (c->graph[k]) { cudaGraphExecDestroy(c->graph[k]); c->graph[k] = nullptr; }
-        if (c->graph_multi[k]) { cudaGraphExecDestroy(c->graph_multi[k]); c->graph_multi[k] = nullptr; }
-        for (int w = 0; w < 2; ++w)
-            if (c->graph_shard[k][w]) { cudaGraphExecDestroy(c->graph_shard[k][w]); c->graph_shard[k][w] = nullptr; }
+        drop(c->graph[k]);
+        drop(c->graph_multi[k]);
+        for (int w = 0; w < 2; ++w) drop(c->graph_shard[k][w]);
     }
 }
 
@@ -383,6 +409,37 @@ int launch_step(SphCtx *c, cudaStream_t st, StageTimer *tm, int64_t *kernels) {
     if (tm) tm->mark(T_TOTAL);
     CUDA_TRY(c, cudaGetLastError());
     c->built = false; c->list_valid = false;  // positions moved
+    return SPH_OK;
+}
+
+// Replay the graph in `slot`, capturing it first if the slot is empty: issue(stream, kernels) launches `span`
+// consecutive steps starting from the current ping-pong parity.  `what` names the graph in error messages.
+template <typename Issue>
+int replay_graph(SphCtx *ctx, cudaStream_t st, GraphSlot &slot, int span, cudaStreamCaptureMode mode, const char *what,
+                 Issue issue) {
+    const int par = ctx->parity;
+    if (!slot.exec) {
+        cudaGraph_t g = nullptr;
+        int64_t kernels = 0;
+        if (!ctx->capture_stream) CUDA_TRY(ctx, cudaStreamCreateWithFlags(&ctx->capture_stream, cudaStreamNonBlocking));
+        cudaStream_t cs = ctx->capture_stream;
+        CUDA_TRY(ctx, cudaStreamBeginCapture(cs, mode));
+        const int rc = issue(cs, &kernels);
+        cudaError_t e = cudaStreamEndCapture(cs, &g);
+        // capture advanced the host-side parity exactly as real steps do; rewind
+        ctx->parity = par;
+        bind_arrays(ctx);
+        if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+        if (e != cudaSuccess) return fail(ctx, SPH_E_CUDA, std::string(what) + " capture: " + cudaGetErrorString(e));
+        e = cudaGraphInstantiate(&slot.exec, g, 0);
+        cudaGraphDestroy(g);
+        if (e != cudaSuccess) return fail(ctx, SPH_E_CUDA, std::string(what) + " instantiate: " + cudaGetErrorString(e));
+        slot.kernels = kernels;
+    }
+    CUDA_TRY(ctx, cudaGraphLaunch(slot.exec, st));
+    ctx->launches += slot.kernels;
+    if (span & 1) { ctx->parity = par ^ 1; bind_arrays(ctx); }
+    ctx->built = false; ctx->list_valid = false;  // positions moved
     return SPH_OK;
 }
 
@@ -660,29 +717,6 @@ int sph_solve_constraints(SphCtx *ctx, int32_t body, float *R_out_dev, void *str
     return rigid_call(ctx, body, 2, R_out_dev, stream);
 }
 
-// Capture `nsteps` consecutive steps (starting from the current ping-pong parity) into one graph.
-static int capture_steps(SphCtx *ctx, int nsteps, cudaGraphExec_t *out, int64_t *kernels_out) {
-    const int par = ctx->parity;
-    cudaGraph_t g = nullptr;
-    int64_t kernels = 0;
-    if (!ctx->capture_stream) CUDA_TRY(ctx, cudaStreamCreateWithFlags(&ctx->capture_stream, cudaStreamNonBlocking));
-    cudaStream_t cs = ctx->capture_stream;
-    CUDA_TRY(ctx, cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-    int rc = SPH_OK;
-    for (int s = 0; s < nsteps && rc == SPH_OK; ++s) rc = launch_step(ctx, cs, nullptr, &kernels);
-    cudaError_t e = cudaStreamEndCapture(cs, &g);
-    // capture advanced the host-side parity exactly as real steps do; rewind
-    ctx->parity = par;
-    bind_arrays(ctx);
-    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-    if (e != cudaSuccess) return fail(ctx, SPH_E_CUDA, std::string("graph capture: ") + cudaGetErrorString(e));
-    e = cudaGraphInstantiate(out, g, 0);
-    cudaGraphDestroy(g);
-    if (e != cudaSuccess) return fail(ctx, SPH_E_CUDA, std::string("graph instantiate: ") + cudaGetErrorString(e));
-    *kernels_out = kernels;
-    return SPH_OK;
-}
-
 int sph_get_rigid_state(SphCtx *ctx, int32_t body, float *out_dev12, void *stream) {
     if (!ctx || !out_dev12) return SPH_E_ARG;
     if (body < 0 || body >= (int)ctx->bodies.size()) return fail(ctx, SPH_E_ARG, "rigid body index out of range");
@@ -699,20 +733,17 @@ int sph_step(SphCtx *ctx, int32_t nsteps, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int s = 0;
     while (s < nsteps) {
-        const int par = ctx->parity;
-        // GRAPH_UNROLL (even) steps per replay amortise the graph-launch gap; the parity returns to `par`
+        // GRAPH_UNROLL (even) steps per replay amortise the graph-launch gap; the parity returns to its start
         const bool multi = nsteps - s >= GRAPH_UNROLL;
-        cudaGraphExec_t *slot = multi ? &ctx->graph_multi[par] : &ctx->graph[par];
-        int64_t *kslot = multi ? &ctx->graph_multi_kernels[par] : &ctx->graph_kernels[par];
         const int span = multi ? GRAPH_UNROLL : 1;
-        if (!*slot) {
-            int rc = capture_steps(ctx, span, slot, kslot);
-            if (rc) return rc;
-        }
-        CUDA_TRY(ctx, cudaGraphLaunch(*slot, st));
-        ctx->launches += *kslot;
-        if (span & 1) { ctx->parity = par ^ 1; bind_arrays(ctx); }
-        ctx->built = false; ctx->list_valid = false;
+        GraphSlot &slot = multi ? ctx->graph_multi[ctx->parity] : ctx->graph[ctx->parity];
+        int rc = replay_graph(ctx, st, slot, span, cudaStreamCaptureModeThreadLocal, "graph",
+                              [&](cudaStream_t cs, int64_t *kernels) {
+                                  int rc = SPH_OK;
+                                  for (int k = 0; k < span && rc == SPH_OK; ++k) rc = launch_step(ctx, cs, nullptr, kernels);
+                                  return rc;
+                              });
+        if (rc) return rc;
         s += span;
     }
     return SPH_OK;
@@ -755,37 +786,51 @@ int nccl_recv(void *user, void *buf, uint64_t bytes, int32_t peer, void *stream)
     } while (0)
 #endif
 
+// One send + recv of `bytes` with `peer` inside a transport group; counts the bytes this rank sent.
+int xfer_pair(SphCtx *c, cudaStream_t st, int peer, const void *sp, void *rp, uint64_t bytes) {
+    const SphTransport t = c->transport;
+    TRANSPORT_OP(st, t.send(t.user, sp, bytes, peer, st));
+    TRANSPORT_OP(st, t.recv(t.user, rp, bytes, peer, st));
+    c->xfer_bytes += bytes;
+    return SPH_OK;
+}
+
+// One transport group: per_side(side, peer) for each neighbour this rank has (side 0 = rank - 1, side 1 = rank + 1),
+// then tail(), both issuing their messages through xfer_pair.
+template <typename PerSide, typename Tail>
+int transport_group(SphCtx *c, cudaStream_t st, PerSide per_side, Tail tail) {
+    if (!c->has_transport) return fail(c, SPH_E_ARG, "no transport: call sph_comm_init_nccl or sph_comm_set_transport first");
+    const SphTransport t = c->transport;
+    TRANSPORT_OP(st, t.group_start(t.user));
+    c->xfer_groups += 1;
+    for (int side = 0; side < 2; ++side) {
+        const int peer = side == 0 ? c->rank - 1 : c->rank + 1;
+        if (peer < 0 || peer >= c->world) continue;
+        if (int rc = per_side(side, peer)) return rc;
+    }
+    if (int rc = tail()) return rc;
+    TRANSPORT_OP(st, t.group_end(t.user, st));
+    return SPH_OK;
+}
+
 // One halo exchange: the packed staging of both sides goes out, the neighbours' records land behind the live
 // records of the CURRENT buffer set (left neighbour's at n - 2 * halo_cap, right neighbour's at n - halo_cap),
 // their headers in the device step state.  Fixed-size messages (the record count travels in the header), so the
 // whole group can be captured in a CUDA graph.
 int shard_exchange(SphCtx *c, cudaStream_t st, bool wide) {
     if (c->world <= 1) return SPH_OK;
-    if (!c->has_transport) return fail(c, SPH_E_ARG, "no transport: call sph_comm_init_nccl or sph_comm_set_transport first");
-    const SphTransport t = c->transport;
     const DevArrays S = c->S;
     const uint64_t bytes = (uint64_t)(wide ? c->P.halo_cap : c->narrow_cap) * 16;
     float4 *cur[4] = {S.posm, S.veld, S.x0id, S.misc};
-    TRANSPORT_OP(st, t.group_start(t.user));
-    c->xfer_groups += 1;
-    for (int side = 0; side < 2; ++side) {
-        const int peer = side == 0 ? c->rank - 1 : c->rank + 1;
-        if (peer < 0 || peer >= c->world) continue;
-        c->xfer_bytes += 4 * bytes + 64;
-        const int64_t tail = (int64_t)c->P.n - (side == 0 ? 2 : 1) * (int64_t)c->P.halo_cap;
-        for (int k = 0; k < 4; ++k) {
-            const void *sp = S.stage[side][k];
-            void *rp = cur[k] + tail;
-            TRANSPORT_OP(st, t.send(t.user, sp, bytes, peer, st));
-            TRANSPORT_OP(st, t.recv(t.user, rp, bytes, peer, st));
-        }
-        const void *hs = S.stage_hdr[side];
-        void *hr = S.sd + (side == 0 ? SD_HDR_L : SD_HDR_R);
-        TRANSPORT_OP(st, t.send(t.user, hs, 64, peer, st));
-        TRANSPORT_OP(st, t.recv(t.user, hr, 64, peer, st));
-    }
-    TRANSPORT_OP(st, t.group_end(t.user, st));
-    return SPH_OK;
+    return transport_group(
+        c, st,
+        [&](int side, int peer) {
+            const int64_t tail = (int64_t)c->P.n - (side == 0 ? 2 : 1) * (int64_t)c->P.halo_cap;
+            for (int k = 0; k < 4; ++k)
+                if (int rc = xfer_pair(c, st, peer, S.stage[side][k], cur[k] + tail, bytes)) return rc;
+            return xfer_pair(c, st, peer, S.stage_hdr[side], S.sd + (side == 0 ? SD_HDR_L : SD_HDR_R), SHARD_HDR_BYTES);
+        },
+        [] { return SPH_OK; });
 }
 
 // plan -> classify + sort -> info -> boundary densities -> boundary forces (-> staging) ->
@@ -843,27 +888,6 @@ int shard_sequence(SphCtx *c, cudaStream_t st, bool compute, bool wide, int64_t 
     if (ev) cudaEventRecord(ev[4], st);
     CUDA_TRY(c, cudaGetLastError());
     c->built = false; c->list_valid = false;
-    return SPH_OK;
-}
-
-int capture_shard_step(SphCtx *ctx, bool wide, cudaGraphExec_t *out, int64_t *kernels_out) {
-    const int par = ctx->parity;
-    cudaGraph_t g = nullptr;
-    int64_t kernels = 0;
-    if (!ctx->capture_stream) CUDA_TRY(ctx, cudaStreamCreateWithFlags(&ctx->capture_stream, cudaStreamNonBlocking));
-    cudaStream_t cs = ctx->capture_stream;
-    // relaxed: NCCL may issue CUDA calls of its own while its send / recv kernels are being captured
-    CUDA_TRY(ctx, cudaStreamBeginCapture(cs, cudaStreamCaptureModeRelaxed));
-    int rc = shard_sequence(ctx, cs, /*compute=*/true, wide, &kernels);
-    cudaError_t e = cudaStreamEndCapture(cs, &g);
-    ctx->parity = par;  // capture advanced the host-side parity exactly as a real step does; rewind
-    bind_arrays(ctx);
-    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-    if (e != cudaSuccess) return fail(ctx, SPH_E_CUDA, std::string("sharded graph capture: ") + cudaGetErrorString(e));
-    e = cudaGraphInstantiate(out, g, 0);
-    cudaGraphDestroy(g);
-    if (e != cudaSuccess) return fail(ctx, SPH_E_CUDA, std::string("sharded graph instantiate: ") + cudaGetErrorString(e));
-    *kernels_out = kernels;
     return SPH_OK;
 }
 
@@ -931,14 +955,12 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
     const int32_t n_mine = ctx->P.n;
     drop_graphs(ctx);
     if (ctx->shard_buf) { cudaFree(ctx->shard_buf); ctx->shard_buf = nullptr; }
-    // {state ints | 2 headers | staging | DFSPH: DX ranges + alignment headers | one fp64 error partial per rank}
-    const uint64_t bytes = 256 + 2 * 256 + 8 * align_up((uint64_t)halo_capacity * 16, 256) + 256 +
-                           align_up((uint64_t)ctx->world * 8, 256);
-    CUDA_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->shard_buf), bytes));
-    CUDA_TRY(ctx, cudaMemset(ctx->shard_buf, 0, bytes));
+    ctx->SL = make_shard_layout(halo_capacity, ctx->world);
+    CUDA_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->shard_buf), ctx->SL.total));
+    CUDA_TRY(ctx, cudaMemset(ctx->shard_buf, 0, ctx->SL.total));
     int32_t sd[SD_INTS] = {0};
     sd[SD_N_LIVE] = n_mine; sd[SD_OWNED] = n_mine; sd[SD_SX0] = x_lo; sd[SD_SX1] = x_hi;
-    CUDA_TRY(ctx, cudaMemcpy(ctx->shard_buf, sd, sizeof(sd), cudaMemcpyHostToDevice));
+    CUDA_TRY(ctx, cudaMemcpy(ctx->shard_buf + ctx->SL.off_state, sd, sizeof(sd), cudaMemcpyHostToDevice));
     ctx->P.slab_on = 1; ctx->P.sgw = ghost_layers; ctx->P.halo_cap = (int32_t)halo_capacity;
     ctx->P.has_left = ctx->rank > 0; ctx->P.has_right = ctx->rank + 1 < ctx->world;
     ctx->P.rebalance_every = rebalance_every;
@@ -1004,21 +1026,12 @@ int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream) {
     static const bool eager = !(std::getenv("SPH_SHARD_GRAPH") && std::atoi(std::getenv("SPH_SHARD_GRAPH")) != 0);
     for (int s = 0; s < nsteps; ++s) {
         const bool wide = shard_wide(ctx);
-        if (eager) {
-            int rc = shard_sequence(ctx, st, /*compute=*/true, wide, &ctx->launches);
-            if (rc) return rc;
-            ctx->shard_sequences += 1;
-            continue;
-        }
-        const int par = ctx->parity;
-        if (!ctx->graph_shard[par][wide]) {
-            int rc = capture_shard_step(ctx, wide, &ctx->graph_shard[par][wide], &ctx->graph_shard_kernels[par][wide]);
-            if (rc) return rc;
-        }
-        CUDA_TRY(ctx, cudaGraphLaunch(ctx->graph_shard[par][wide], st));
-        ctx->launches += ctx->graph_shard_kernels[par][wide];
-        ctx->parity = par ^ 1;
-        bind_arrays(ctx);
+        auto issue = [&](cudaStream_t cs, int64_t *kernels) { return shard_sequence(ctx, cs, /*compute=*/true, wide, kernels); };
+        // relaxed capture: NCCL may issue CUDA calls of its own while its send / recv kernels are being captured
+        int rc = eager ? issue(st, &ctx->launches)
+                       : replay_graph(ctx, st, ctx->graph_shard[ctx->parity][wide], 1, cudaStreamCaptureModeRelaxed,
+                                      "sharded graph", issue);
+        if (rc) return rc;
         ctx->shard_sequences += 1;
     }
     return SPH_OK;
@@ -1114,12 +1127,9 @@ int sph_dfsph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream
 }  // extern "C"
 namespace {
 
-// Sharded DFSPH blocks of the shard buffer, behind the staging: the DX_* ranges + alignment headers (256 B), then one
-// fp64 error partial per rank
-inline int32_t *shard_dx(const SphCtx *c) {
-    return reinterpret_cast<int32_t *>(c->shard_buf + 768 + 8 * align_up((uint64_t)c->P.halo_cap * 16, 256));
-}
-inline double *shard_err_parts(const SphCtx *c) { return reinterpret_cast<double *>(shard_dx(c) + DX_INTS); }
+// Sharded DFSPH blocks of the shard buffer: the DX_* ranges + alignment headers, and one fp64 error partial per rank
+inline int32_t *shard_dx(const SphCtx *c) { return reinterpret_cast<int32_t *>(c->shard_buf + c->SL.off_dx); }
+inline double *shard_err_parts(const SphCtx *c) { return reinterpret_cast<double *>(c->shard_buf + c->SL.off_err); }
 
 // One exchange of the sharded DFSPH step with both neighbours: pack -> one transport group -> unpack.
 //   DX_ALIGN: the ghost alignment (4 record arrays of the sgw boundary layers + a 16-byte header per side), received
@@ -1130,11 +1140,9 @@ inline double *shard_err_parts(const SphCtx *c) { return reinterpret_cast<double
 // same group also sends this rank's fp64 error partial (ctrl->err) to every other rank and receives theirs into
 // shard_err_parts() -- an all-gather of 8 bytes with plain send / recv.  ctrl (may be NULL): the pack and unpack of a
 // sweep behind the converged one return at once, but its transport calls are still issued, so that every rank issues
-// the same sequence.
+// the same sequence.  Returns at once on a context that is not sharded or has no neighbours.
 int shard_dfsph_exchange(SphCtx *c, cudaStream_t st, int what, DfsphCtrl *ctrl, bool gather_err, int64_t *kernels) {
-    if (c->world <= 1) return SPH_OK;
-    if (!c->has_transport) return fail(c, SPH_E_ARG, "no transport: call sph_comm_init_nccl or sph_comm_set_transport first");
-    const SphTransport t = c->transport;
+    if (c->world <= 1 || !c->P.slab_on) return SPH_OK;
     const DevArrays S = c->S;
     const DevParams &P = c->P;
     int32_t *dx = shard_dx(c);
@@ -1150,37 +1158,22 @@ int shard_dfsph_exchange(SphCtx *c, cudaStream_t st, int what, DfsphCtrl *ctrl, 
     const dim3 grid(blocks_for(cap, 256), 2);
     k_dfsph_shard_pack<<<grid, 256, 0, st>>>(P, S, dx, what, ctrl);
     CUDA_TRY(c, cudaGetLastError());
-    TRANSPORT_OP(st, t.group_start(t.user));
-    c->xfer_groups += 1;
-    for (int side = 0; side < 2; ++side) {
-        const int peer = side == 0 ? c->rank - 1 : c->rank + 1;
-        if (peer < 0 || peer >= c->world) continue;
-        for (int k = 0; k < narr; ++k) {
-            const void *sp = S.stage[side][k];
-            void *rp = rec[side][k];
-            TRANSPORT_OP(st, t.send(t.user, sp, bytes, peer, st));
-            TRANSPORT_OP(st, t.recv(t.user, rp, bytes, peer, st));
-        }
-        c->xfer_bytes += narr * bytes;
-        if (what == DX_ALIGN) {
-            const void *hs = dx + DX_HDR_SEND + 4 * side;
-            void *hr = dx + DX_HDR_RECV + 4 * side;
-            TRANSPORT_OP(st, t.send(t.user, hs, 16, peer, st));
-            TRANSPORT_OP(st, t.recv(t.user, hr, 16, peer, st));
-            c->xfer_bytes += 16;
-        }
-    }
-    if (gather_err) {
-        for (int r = 0; r < c->world; ++r) {
-            if (r == c->rank) continue;
-            const void *es = &ctrl->err;
-            void *er = parts + r;
-            TRANSPORT_OP(st, t.send(t.user, es, 8, r, st));
-            TRANSPORT_OP(st, t.recv(t.user, er, 8, r, st));
-            c->xfer_bytes += 8;
-        }
-    }
-    TRANSPORT_OP(st, t.group_end(t.user, st));
+    int rc = transport_group(
+        c, st,
+        [&](int side, int peer) {
+            for (int k = 0; k < narr; ++k)
+                if (int rc = xfer_pair(c, st, peer, S.stage[side][k], rec[side][k], bytes)) return rc;
+            if (what != DX_ALIGN) return SPH_OK;
+            return xfer_pair(c, st, peer, dx + DX_HDR_SEND + 4 * side, dx + DX_HDR_RECV + 4 * side, 16);
+        },
+        [&] {
+            for (int r = 0; gather_err && r < c->world; ++r) {
+                if (r == c->rank) continue;
+                if (int rc = xfer_pair(c, st, r, &ctrl->err, parts + r, 8)) return rc;
+            }
+            return SPH_OK;
+        });
+    if (rc) return rc;
     k_dfsph_shard_unpack<<<grid, 256, 0, st>>>(P, S, dx, what, ctrl, rec[0][0], rec[0][1], rec[0][2], rec[0][3], rec[1][0],
                                                rec[1][1], rec[1][2], rec[1][3]);
     *kernels += 2;
@@ -1196,35 +1189,31 @@ int shard_dfsph_exchange(SphCtx *c, cudaStream_t st, int what, DfsphCtrl *ctrl, 
 // {factor, density_adv} after the density change to the neighbours' first ghost layer, and all-gathers the error
 // partials for k_dfsph_check_ranked; n_fluid is then the global fluid count.
 int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, float offset, int64_t n_fluid,
-                     int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t n_grid = -1) {
+                     int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
     const DevParams &P = ctx->P;
     DfsphCtrl *ctrl = reinterpret_cast<DfsphCtrl *>(ctx->ws + ctx->L.off_scratch);
     *h = DfsphCtrl{};
     CUDA_TRY(ctx, cudaMemsetAsync(ctrl, 0, sizeof(DfsphCtrl), st));
     if (P.n == 0) return SPH_OK;
-    const bool shard = P.slab_on != 0;
-    const int b128 = blocks_for(n_grid < 0 ? P.n : n_grid, 128);
+    const int b128 = blocks_for(n_grid, 128);
     int batch = std::max(1, std::min(first_batch, 64));
     while (!h->done) {
         for (int s = 0; s < batch; ++s) {
             if (mode == 0) k_dfsph_iteration<0><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
             else k_dfsph_iteration<1><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
-            if (shard) {
-                int rc = shard_dfsph_exchange(ctx, st, DX_VELD, ctrl, false, &ctx->launches);
-                if (rc) return rc;
-            }
+            int rc = shard_dfsph_exchange(ctx, st, DX_VELD, ctrl, false, kernels);
+            if (rc) return rc;
             if (mode == 0) k_dfsph_density_change_err<0><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
             else k_dfsph_density_change_err<1><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
-            if (shard) {
-                int rc = shard_dfsph_exchange(ctx, st, DX_DFS, ctrl, true, &ctx->launches);
-                if (rc) return rc;
+            rc = shard_dfsph_exchange(ctx, st, DX_DFS, ctrl, true, kernels);
+            if (rc) return rc;
+            if (P.slab_on)
                 k_dfsph_check_ranked<<<1, 1, 0, st>>>(ctrl, shard_err_parts(ctx), ctx->rank, ctx->world, (double)n_fluid, eta,
                                                       max_iterations);
-            } else {
+            else
                 k_dfsph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
-            }
         }
-        ctx->launches += 3 * (int64_t)batch;
+        *kernels += 3 * (int64_t)batch;
         CUDA_TRY(ctx, cudaGetLastError());
         CUDA_TRY(ctx, cudaMemcpyAsync(h, ctrl, sizeof(DfsphCtrl), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(ctx, cudaStreamSynchronize(st));
@@ -1233,23 +1222,66 @@ int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, 
     return SPH_OK;
 }
 
+// DFSPH.substep (DFSPH.py:399-408) over the sorted records [0, n_grid), with io's constants in and its counts out:
+//   densities -> factor -> [density change -> * 1/dt -> dfs exchange -> divergence loop -> * dt] -> non-pressure
+//   forces -> predict velocity -> veld exchange -> density_adv -> * 1/dt^2 -> dfs exchange -> pressure loop -> advect
+// The exchanges run only on a sharded context.  After its ghost alignment a ghost record holds exactly what its owner
+// holds in the same position, so a value that changes on the owner is sent once per change -- veld after each Jacobi
+// iteration and after predict_velocity, dfs after each density change -- and every pass reads current ghost values.
+// The {factor, density_adv} words are sent AFTER the multiply_time_step that follows each loop's opening density
+// change: one message carries both, and the scale at the end of the divergence loop needs no message because nothing
+// reads a ghost's factor before the pressure loop's opening exchange.
+int launch_dfsph_substep(SphCtx *c, cudaStream_t st, SphDfsphStep *io, int64_t n_grid, int64_t *kernels) {
+    const DevParams &P = c->P;
+    const int b128 = blocks_for(n_grid, 128), b256 = blocks_for(n_grid, 256);
+    launch_pair_density(c, st, kernels, /*split_mode=*/0, n_grid);
+    c->list_valid = true;
+    k_dfsph_factor<<<b128, 128, 0, st>>>(P, c->S);
+    *kernels += 1;
+    DfsphCtrl h{};
+    if (io->enable_divergence_solver) {  // divergence_solve, DFSPH.py:236-276
+        k_dfsph_density_change<0><<<b128, 128, 0, st>>>(P, c->S);
+        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt);
+        *kernels += 2;
+        int rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
+        if (rc) return rc;
+        rc = dfsph_solve_loop(c, 0, io->max_iterations_v, io->eta_v, 0.0f, io->n_fluid, io->first_batch_v, &h, st, n_grid,
+                              kernels);
+        if (rc) return rc;
+        io->iterations_v = h.iterations; io->avg_err_v = h.last_avg; io->first_batch_v = std::max(1, h.sweeps);
+        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->dt);
+        *kernels += 1;
+    }
+    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(P, c->S);
+    k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, c->S);
+    *kernels += 2;
+    int rc = shard_dfsph_exchange(c, st, DX_VELD, nullptr, false, kernels);
+    if (rc) return rc;
+    // pressure_solve, DFSPH.py:314-352
+    k_dfsph_density_change<1><<<b128, 128, 0, st>>>(P, c->S);
+    k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt2);
+    *kernels += 2;
+    rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
+    if (rc) return rc;
+    rc = dfsph_solve_loop(c, 1, io->max_iterations, io->eta, io->density0, io->n_fluid, io->first_batch, &h, st, n_grid,
+                          kernels);
+    if (rc) return rc;
+    io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
+    k_dfsph_advect<<<b256, 256, 0, st>>>(P, c->S);
+    *kernels += 1;
+    c->built = false; c->list_valid = false;  // positions moved
+    return SPH_OK;
+}
+
 // One sharded DFSPH SPHBase.step() (fluid + static solids; no overlap of the exchanges with computation):
-//   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> densities (owned + first ghost layer) -> factor
-//   -> [density change -> * 1/dt -> dfs exchange -> divergence loop -> * dt] -> non-pressure forces -> predict velocity
-//   -> veld exchange -> density_adv -> * 1/dt^2 -> dfs exchange -> pressure loop -> advect + clamp (owned)
-//   -> pack the send ranges -> the record exchange that feeds the next step's classification
-// After the alignment a ghost record holds exactly what its owner holds in the same position, so a value that changes
-// on the owner is sent once per change -- veld after each Jacobi iteration and after predict_velocity, dfs after each
-// density change -- and every pass reads current ghost values.  The {factor, density_adv} words are sent AFTER the
-// multiply_time_step that follows each loop's opening density change: one message carries both, and the scale at the
-// end of the divergence loop needs no message because nothing reads a ghost's factor before the pressure loop's
-// opening exchange.
+//   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> substep on owned records + ghosts
+//   -> clamp (owned) -> pack the send ranges -> the record exchange that feeds the next step's classification
 int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, SphDfsphStep *io, bool wide, int64_t *kernels) {
     k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
     *kernels += 1;
     int rc = launch_neighbor_build(c, st, nullptr, kernels, /*move_acc=*/false);
     if (rc) return rc;
-    const DevParams &P = c->P;  // after the build: the array binding changed sides
+    const DevParams &P = c->P;
     k_shard_info<<<1, 32, 0, st>>>(P, c->S, P.sgw + (wide ? 2 : 1), wide ? P.halo_cap : c->narrow_cap);
     k_dfsph_shard_ranges<<<1, 32, 0, st>>>(P, c->S, shard_dx(c), c->align_cap, c->sweep_cap);
     *kernels += 2;
@@ -1262,49 +1294,15 @@ int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, SphDfsphStep *io, bool wide
     CUDA_TRY(c, cudaMemcpyAsync(&n_live, c->S.sd + SD_N_LIVE, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(c, cudaStreamSynchronize(st));
     const int64_t n_grid = std::min<int64_t>(std::max<int32_t>(n_live, 1), P.n);
-    const int b128 = blocks_for(n_grid, 128), b256 = blocks_for(n_grid, 256);
-    // substep (DFSPH.py:399-408)
-    launch_pair_density(c, st, kernels, /*split_mode=*/0, n_grid);
-    c->list_valid = true;
-    k_dfsph_factor<<<b128, 128, 0, st>>>(P, c->S);
-    *kernels += 1;
-    DfsphCtrl h{};
-    if (io->enable_divergence_solver) {  // divergence_solve, DFSPH.py:236-276
-        k_dfsph_density_change<0><<<b128, 128, 0, st>>>(P, c->S);
-        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt);
-        *kernels += 2;
-        rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
-        if (rc) return rc;
-        rc = dfsph_solve_loop(c, 0, io->max_iterations_v, io->eta_v, 0.0f, io->n_fluid, io->first_batch_v, &h, st, n_grid);
-        if (rc) return rc;
-        io->iterations_v = h.iterations; io->avg_err_v = h.last_avg; io->first_batch_v = std::max(1, h.sweeps);
-        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->dt);
-        *kernels += 1;
-    }
-    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(P, c->S);
-    k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 2;
-    rc = shard_dfsph_exchange(c, st, DX_VELD, nullptr, false, kernels);
+    rc = launch_dfsph_substep(c, st, io, n_grid, kernels);
     if (rc) return rc;
-    // pressure_solve, DFSPH.py:314-352
-    k_dfsph_density_change<1><<<b128, 128, 0, st>>>(P, c->S);
-    k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt2);
-    *kernels += 2;
-    rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
-    if (rc) return rc;
-    rc = dfsph_solve_loop(c, 1, io->max_iterations, io->eta, io->density0, io->n_fluid, io->first_batch, &h, st, n_grid);
-    if (rc) return rc;
-    io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-    k_dfsph_advect<<<b256, 256, 0, st>>>(P, c->S);
-    k_enforce_boundary<<<b256, 256, 0, st>>>(P, c->S, /*particle_type=*/1);  // enforce_boundary_3D(fluid), sph_base.py:271
+    // enforce_boundary_3D(fluid), sph_base.py:271 (no rigid solve before it: sharded contexts hold static solids only)
+    k_enforce_boundary<<<blocks_for(n_grid, 256), 256, 0, st>>>(P, c->S, /*particle_type=*/1);
     // the advanced records of the send ranges -> staging, then the exchange the next step classifies
     k_shard_apply<<<dim3(blocks_for(P.halo_cap, 256), 2), 256, 0, st>>>(P, c->S, /*copy_all=*/1);
-    *kernels += 3;
+    *kernels += 2;
     CUDA_TRY(c, cudaGetLastError());
-    rc = shard_exchange(c, st, wide);
-    if (rc) return rc;
-    c->built = false; c->list_valid = false;
-    return SPH_OK;
+    return shard_exchange(c, st, wide);
 }
 
 }  // namespace
@@ -1317,7 +1315,8 @@ int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double et
     if (!ctx->built || !ctx->list_valid)
         return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run sph_neighbor_build and op 0 (compute_densities) first");
     DfsphCtrl h{};
-    int rc = dfsph_solve_loop(ctx, mode, max_iterations, eta, offset, n_fluid, first_batch, &h, static_cast<cudaStream_t>(stream));
+    int rc = dfsph_solve_loop(ctx, mode, max_iterations, eta, offset, n_fluid, first_batch, &h,
+                              static_cast<cudaStream_t>(stream), ctx->P.n, &ctx->launches);
     if (rc) return rc;
     if (iterations_out) *iterations_out = h.iterations;
     if (sweeps_out) *sweeps_out = h.sweeps;
@@ -1333,42 +1332,14 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int s = 0; s < nsteps; ++s) {
         // ps.initialize_particle_system(), compute_moving_boundary_volume() (sph_base.py:264-265)
-        int rc = launch_neighbor_build(ctx, st, nullptr, &ctx->launches);
+        int rc = launch_neighbor_build(ctx, st, nullptr, &ctx->launches, /*move_acc=*/true);
         if (rc) return rc;
         if (ctx->has_dynamic_solids) { rc = launch_boundary_volume(ctx, 1, st, &ctx->launches); if (rc) return rc; }
-        const DevParams &P = ctx->P;  // after the build: the array binding changed sides
-        const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
-        // substep (DFSPH.py:399-408)
-        launch_pair_density(ctx, st, &ctx->launches);
-        ctx->list_valid = true;
-        k_dfsph_factor<<<b128, 128, 0, st>>>(P, ctx->S);
-        ctx->launches += 1;
-        DfsphCtrl h{};
-        if (io->enable_divergence_solver) {  // divergence_solve, DFSPH.py:236-276
-            k_dfsph_density_change<0><<<b128, 128, 0, st>>>(P, ctx->S);
-            k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, ctx->S, io->inv_dt);
-            ctx->launches += 2;
-            rc = dfsph_solve_loop(ctx, 0, io->max_iterations_v, io->eta_v, 0.0f, io->n_fluid, io->first_batch_v, &h, st);
-            if (rc) return rc;
-            io->iterations_v = h.iterations; io->avg_err_v = h.last_avg; io->first_batch_v = std::max(1, h.sweeps);
-            k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, ctx->S, io->dt);
-            ctx->launches += 1;
-        }
-        k_dfsph_non_pressure<<<b128, 128, 0, st>>>(P, ctx->S);
-        k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, ctx->S);
-        // pressure_solve, DFSPH.py:314-352
-        k_dfsph_density_change<1><<<b128, 128, 0, st>>>(P, ctx->S);
-        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, ctx->S, io->inv_dt2);
-        ctx->launches += 4;
-        rc = dfsph_solve_loop(ctx, 1, io->max_iterations, io->eta, io->density0, io->n_fluid, io->first_batch, &h, st);
+        rc = launch_dfsph_substep(ctx, st, io, ctx->P.n, &ctx->launches);
         if (rc) return rc;
-        io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-        k_dfsph_advect<<<b256, 256, 0, st>>>(P, ctx->S);
-        ctx->launches += 1;
-        ctx->built = false; ctx->list_valid = false;
         // solve_rigid_body(), enforce_boundary_3D(fluid) (sph_base.py:270-271)
         if (!ctx->bodies.empty()) { rc = launch_rigid_solve(ctx, st, &ctx->launches); if (rc) return rc; }
-        k_enforce_boundary<<<b256, 256, 0, st>>>(P, ctx->S, /*particle_type=*/1);
+        k_enforce_boundary<<<blocks_for(ctx->P.n, 256), 256, 0, st>>>(ctx->P, ctx->S, /*particle_type=*/1);
         ctx->launches += 1;
         CUDA_TRY(ctx, cudaGetLastError());
     }

@@ -225,13 +225,8 @@ class ShardedSimulation:
         self._io = None
         if self.dfsph:
             e.set_dfsph(True)
-            # the constants of DFSPHSolver (DFSPH.py:10-17) and its step(): eta, eta_v and the multiply_time_step factors
-            dt, rho0 = float(cfg.get_cfg("timeStepSize")), float(cfg.get_cfg("density0"))
-            max_error_v, max_error = 0.1, 0.05
-            self._io = _lib.SphDfsphStep(enable_divergence_solver=1, max_iterations_v=100, max_iterations=100,
-                                         eta_v=1.0 / dt * max_error_v * 0.01 * rho0, eta=max_error * 0.01 * rho0,
-                                         inv_dt=1 / dt, dt=dt, inv_dt2=1 / (dt * dt), density0=rho0,
-                                         n_fluid=int(n_fluid), first_batch_v=2, first_batch=3)
+            from .DFSPH import dfsph_step_io
+            self._io = dfsph_step_io(float(cfg.get_cfg("timeStepSize")), float(cfg.get_cfg("density0")), n_fluid)
         # ---- transport: NCCL inside the library (its own communicator), or a caller-supplied one (tests) ----
         if transport is not None:
             self._transport = transport
