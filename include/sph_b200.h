@@ -45,6 +45,7 @@ extern "C" {
 #define SPH_STATUS_SHARD_CAPACITY 8u /* sharded: live + received records ran into the receive regions */
 #define SPH_STATUS_SHARD_VELOCITY 16u /* sharded DFSPH: a particle moved >= one cell layer in x in one step */
 #define SPH_STATUS_GHOST_ALIGN 32u   /* sharded DFSPH: a neighbour's boundary layers and the ghost layers differ */
+#define SPH_STATUS_SOLID_SLOT 64u    /* sharded with dynamic solids: two live records carry the same solid id */
 
 /* Scalar parameters.  All constants are folded in double on the host exactly as the
  * reference folds them in Python scope before Taichi bakes them into kernels
@@ -213,7 +214,8 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
  * rides the exchange like a fluid one (posm.w = its boundary volume m_V, misc = material, flags, solid_id) and is
  * staged unchanged, so the caller must pack every solid with its final start-up m_V -- the value the single engine's
  * sph_boundary_volume computes over the WHOLE scene (a solid's neighbours may sit across a cut).  Dynamic solids
- * (shape-matched bodies, advected rigid blocks) are single-GPU: sph_shard_configure refuses them, and on a sharded
+ * (shape-matched bodies, advected rigid blocks) shard in WCSPH only through sph_shard_configure_bodies (below);
+ * sph_shard_configure refuses them, and on a sharded
  * context sph_set_solid_count refuses the dynamic flag, sph_set_rigid_bodies a body table, and sph_boundary_volume,
  * sph_compute_com, sph_compute_rigid_rest_cm and sph_solve_constraints refuse to run (they walk solid ids through a
  * slot map that migration leaves stale for solids of other ranks).
@@ -245,6 +247,22 @@ int sph_comm_set_transport(SphCtx *ctx, const SphTransport *t, int32_t rank, int
  * side and direction (>= (ghost_layers + 2) fullest layers). */
 int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                         int32_t rebalance_every);
+/* Opt-in sharding of WCSPH scenes with DYNAMIC solids: shape-matched bodies (`bodies`, solid-id ranges of the WHOLE
+ * scene's ids, rest_cm computed over the whole scene; n_bodies = 0: advected rigid blocks only) and advected rigid
+ * blocks.  Pack first (sph_set_solid_count with the whole scene's solid count and the dynamic flag, uniform fluid);
+ * needs ghost_layers >= 3 (a moving solid's m_V in the second ghost layer sums solids of the third).  DFSPH contexts
+ * are refused.  sph_shard_step then runs, eagerly on `stream` (no overlap, SPH_SHARD_GRAPH does not apply):
+ *     plan -> sort -> info -> solid-id slot map of the live records (SPH_STATUS_SOLID_SLOT on a duplicate id)
+ *     -> moving boundary volumes of the owned layers and ghost layers 1-2 -> densities -> forces + integration of
+ *     the owned fluid -> the fluid's reactions GATHERED onto each owned dynamic solid (fluid of the owned layers and
+ *     ghost layer 1) + its advection -> {x, m} and x_0 of the owned body particles -> all-gather of those records
+ *     (one transport group, (world - 1) * 32 bytes per body particle sent) -> sph_step's shape matching (the same
+ *     fp32 reduction in the same order) on every rank, and clamps -> the record exchange.
+ * cm and R are bit-identical on every rank (sph_get_rigid_state works on every rank) and equal to the single
+ * engine's for the same particle positions; ghost copies catch up through the record exchange.  The body table is fixed: sph_set_rigid_bodies, the per-body calls, sph_boundary_volume,
+ * sph_shard_profile_step and sph_shard_dfsph_step are refused on such a context. */
+int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                               int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies);
 /* first sort of the packed particles + the first halo exchange (no physics) */
 int sph_shard_begin(SphCtx *ctx, void *stream);
 /* nsteps sharded SPHBase.step()s (sph_base.py:263-271): asynchronous launches that run ahead of the device (no host

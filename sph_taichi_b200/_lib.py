@@ -27,7 +27,7 @@ ABI_SYMBOLS = [
     "sph_launch_count", "sph_profile_step", "sph_timer_name", "sph_state_offsets", "sph_set_dfsph", "sph_dfsph_op", "sph_dfsph_solve", "sph_dfsph_step",
     "sph_comm_unique_id", "sph_comm_init_nccl", "sph_comm_set_transport", "sph_shard_configure", "sph_shard_begin",
     "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step", "sph_shard_dfsph_step",
-    "sph_shard_transport_stats",
+    "sph_shard_transport_stats", "sph_shard_configure_bodies",
 ]
 
 
@@ -153,6 +153,7 @@ def load():
         "sph_comm_init_nccl": (C.c_int, [vp, C.c_char_p, i32, i32]),
         "sph_comm_set_transport": (C.c_int, [vp, C.POINTER(SphTransport), i32, i32]),
         "sph_shard_configure": (C.c_int, [vp, i32, i32, i32, i64, i32]),
+        "sph_shard_configure_bodies": (C.c_int, [vp, i32, i32, i32, i64, i32, C.POINTER(SphRigidBody), i32]),
         "sph_shard_begin": (C.c_int, [vp, vp]),
         "sph_shard_step": (C.c_int, [vp, i32, vp]),
         "sph_halo_exchange": (C.c_int, [vp, vp]),

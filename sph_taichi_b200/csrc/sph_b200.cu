@@ -20,12 +20,18 @@ namespace {
 
 std::string g_create_error;
 
-// Sharded contexts hold static solids only.  The solid-id slot map of a rank is not reset or validated under
+// Contexts configured by sph_shard_configure hold static solids only.  The solid-id slot map of a rank is not reset or validated under
 // migration (a trash-bucket record may share its id with a live one, a solid on another rank leaves its slot stale),
 // so every entry point that walks it -- boundary volumes, advect-solids, the rigid-body calls -- is refused there.
 const char *const kShardStaticOnly =
     "x-slab sharding supports static solids only: dynamic solids (shape-matched bodies, advected rigid blocks) and "
     "the rigid-body and boundary-volume calls that walk solid ids are single-GPU in WCSPH and DFSPH";
+// sph_shard_configure_bodies (opt-in, WCSPH): the step re-validates the slot map and solves the bodies across ranks
+const char *const kShardBodiesWcsph =
+    "x-slab sharding of dynamic solids is WCSPH only: the DFSPH pressure sweeps scatter the reactions onto the bodies "
+    "in every sweep, which would need a reaction exchange per sweep";
+const char *const kShardBodiesFixed =
+    "the body table of a context configured by sph_shard_configure_bodies is fixed: configure a new context";
 
 constexpr int NUM_TIMERS = 12;
 constexpr int GRAPH_UNROLL = 4;  // must be even (ping-pong parity returns to its start)
@@ -79,13 +85,14 @@ Layout make_layout(int64_t n_max, int64_t C, int64_t n_solid, int n_bodies) {
 constexpr uint64_t SHARD_HDR_BYTES = 64;  // the 16-int header that travels with every record exchange
 
 // The shard buffer (library-owned, x-slab sharding): {device step state | send header x 2 | 2 sides x 4 send staging
-// arrays x halo_cap records | sharded DFSPH: DX ranges + alignment headers | one fp64 error partial per rank}
+// arrays x halo_cap records | sharded DFSPH: DX ranges + alignment headers | one fp64 error partial per rank
+// [| with shape-matched bodies: every rank's table of the body particles' records, 2 x 16 bytes per body particle]}
 struct ShardLayout {
-    uint64_t off_state, off_hdr[2], off_stage[2][4], off_dx, off_err;
+    uint64_t off_state, off_hdr[2], off_stage[2][4], off_dx, off_err, off_body;
     uint64_t total;
 };
 
-ShardLayout make_shard_layout(int64_t halo_cap, int world) {
+ShardLayout make_shard_layout(int64_t halo_cap, int world, int64_t n_body_particles = 0) {
     ShardLayout L;
     uint64_t o = 0;
     auto take = [&](uint64_t bytes) { uint64_t r = o; o = align_up(o + bytes, 256); return r; };
@@ -95,6 +102,7 @@ ShardLayout make_shard_layout(int64_t halo_cap, int world) {
         for (int k = 0; k < 4; ++k) L.off_stage[side][k] = take((uint64_t)halo_cap * 16);
     L.off_dx = take(DX_INTS * 4);
     L.off_err = take((uint64_t)world * 8);
+    L.off_body = n_body_particles > 0 ? take((uint64_t)world * n_body_particles * 32) : 0;
     L.total = o;
     return L;
 }
@@ -190,6 +198,7 @@ struct SphCtx {
     // sharded DFSPH: records per side of the ghost alignment (sgw layers) and of a per-sweep exchange (one layer)
     int32_t align_cap = 0, sweep_cap = 0;
     int shard_world = 1;  // world size the shard buffer's per-rank error partials were sized for
+    bool shard_bodies = false;  // configured by sph_shard_configure_bodies: steps with shard_bodies_sequence
     uint64_t xfer_groups = 0, xfer_bytes = 0;  // transport groups issued from the host, and the bytes this rank sent
 };
 
@@ -256,6 +265,9 @@ void bind_arrays(SphCtx *c) {
 }
 
 inline RigidBodyDev *dev_bodies(SphCtx *c) { return reinterpret_cast<RigidBodyDev *>(c->ws + c->L.off_bodies); }
+int store_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodies);
+int shard_setup(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                int32_t rebalance_every, int64_t n_body_particles);
 
 inline int blocks_for(int64_t n, int t) { return (int)((n + t - 1) / t); }
 // Sharded steps: n is the capacity and the real counts are device state, so the LIGHT step kernels (histogram,
@@ -373,7 +385,7 @@ void launch_pair_force_and_advect(SphCtx *c, cudaStream_t st, StageTimer *tm, in
 int launch_boundary_volume(SphCtx *c, int moving, cudaStream_t st, int64_t *kernels) {
     const DevParams &P = c->P;
     if (P.n_solid == 0) return SPH_OK;
-    k_boundary_volume<<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S, moving);
+    k_boundary_volume<false><<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S, moving);
     *kernels += 1;
     CUDA_TRY(c, cudaGetLastError());
     return SPH_OK;
@@ -386,7 +398,7 @@ int launch_rigid_solve(SphCtx *c, cudaStream_t st, int64_t *kernels) {
     const int nb = (int)c->bodies.size();
     if (nb == 0) return SPH_OK;
     k_rigid<<<nb, RIGID_THREADS, 0, st>>>(c->P, c->S, dev_bodies(c), 0, 2, nullptr, nb);
-    k_enforce_boundary_solid<<<blocks_for(c->P.n_solid, 256), 256, 0, st>>>(c->P, c->S, nb, dev_bodies(c), nb);
+    k_enforce_boundary_solid<false><<<blocks_for(c->P.n_solid, 256), 256, 0, st>>>(c->P, c->S, nb, dev_bodies(c), nb);
     *kernels += 2;
     CUDA_TRY(c, cudaGetLastError());
     return SPH_OK;
@@ -679,9 +691,17 @@ int sph_set_rigid_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodi
     if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
     if (n_bodies > ctx->body_cap) return fail(ctx, SPH_E_CAPACITY, "more rigid bodies than the workspace was sized for");
     if (ctx->P.slab_on && n_bodies > 0) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
+    if (ctx->shard_bodies) return fail(ctx, SPH_E_ARG, kShardBodiesFixed);
     for (int b = 0; b < n_bodies; ++b)  // validate everything before any state changes
         if (bodies[b].solid_begin < 0 || bodies[b].solid_end < bodies[b].solid_begin || bodies[b].solid_end > ctx->n_solid_cap)
             return fail(ctx, SPH_E_ARG, "rigid body solid-id range out of bounds");
+    return store_bodies(ctx, bodies, n_bodies);
+}
+
+}  // extern "C"
+namespace {
+// The body table on the host and on the device (R = I, cm = 0 until the first solve).
+int store_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodies) {
     ctx->bodies.assign(bodies, bodies + n_bodies);
     std::vector<RigidBodyDev> h(n_bodies);
     for (int b = 0; b < n_bodies; ++b) {
@@ -696,6 +716,8 @@ int sph_set_rigid_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodi
     drop_graphs(ctx);
     return SPH_OK;
 }
+}  // namespace
+extern "C" {
 
 static int rigid_call(SphCtx *ctx, int32_t body, int mode, float *out, void *stream) {
     if (!ctx) return SPH_E_ARG;
@@ -891,6 +913,82 @@ int shard_sequence(SphCtx *c, cudaStream_t st, bool compute, bool wide, int64_t 
     return SPH_OK;
 }
 
+inline float4 *shard_body_tables(const SphCtx *c) { return reinterpret_cast<float4 *>(c->shard_buf + c->SL.off_body); }
+inline int64_t body_particles(const std::vector<SphRigidBody> &bodies) {
+    int64_t n = 0;
+    for (const SphRigidBody &b : bodies) n += b.solid_end - b.solid_begin;
+    return n;
+}
+
+// One sharded WCSPH SPHBase.step() with dynamic solids (sph_shard_configure_bodies), in the order of launch_step +
+// launch_rigid_solve, on one stream and without overlap:
+//   plan -> classify + sort -> info -> solid-id slot map -> moving boundary volumes (owned + ghost layers 1-2)
+//   -> densities (owned + ghost layer 1) -> forces + integration of the owned fluid (no reaction scatter)
+//   -> reactions gathered onto the owned dynamic solids + their advection -> body-particle records -> all-gather ->
+//   k_rigid's solve + clamps on every rank -> clamps of the other dynamic solids -> pack the send ranges -> the record
+//   exchange
+int shard_bodies_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels) {
+    k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+    int rc = launch_neighbor_build(c, st, nullptr, kernels, /*move_acc=*/false);
+    if (rc) return rc;
+    const DevParams &P = c->P;
+    k_shard_info<<<1, 32, 0, st>>>(P, c->S, P.sgw + (wide ? 2 : 1), wide ? P.halo_cap : c->narrow_cap);
+    *kernels += 1;
+    if (P.n_solid > 0) {
+        // k_rank_move also wrote the slots of trash records: only the live ones may be walked
+        CUDA_TRY(c, cudaMemsetAsync(c->S.solid_slot, 0xff, (size_t)P.n_solid * 4, st));
+        k_shard_solid_slots<<<step_grid(c, P.n, 256, 8), 256, 0, st>>>(P, c->S);
+        *kernels += 1;
+        if (c->has_dynamic_solids) {
+            k_boundary_volume<true><<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S, /*moving=*/1);
+            *kernels += 1;
+        }
+    }
+    launch_pair_density(c, st, kernels, /*split_mode=*/0);
+    PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS, true, true>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st,
+               P, c->S, 0);
+    *kernels += 1;
+    CUDA_TRY(c, cudaGetLastError());
+    const int nb = (int)c->bodies.size();
+    if (P.n_solid > 0) {
+        k_shard_reactions<<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S);
+        *kernels += 1;
+    }
+    if (nb > 0) {
+        // k_rigid's solve on every rank: the records of all body particles, gathered, in one transport group
+        const int64_t n_rec = body_particles(c->bodies);
+        float4 *tables = shard_body_tables(c);
+        float4 *mine = tables + 2 * (size_t)c->rank * n_rec;
+        k_shard_body_pack<<<nb, 256, 0, st>>>(P, c->S, dev_bodies(c), mine);
+        *kernels += 1;
+        CUDA_TRY(c, cudaGetLastError());
+        if (c->world > 1) {
+            const uint64_t bytes = (uint64_t)n_rec * 32;
+            rc = transport_group(
+                c, st, [](int, int) { return SPH_OK; },
+                [&] {
+                    for (int r = 0; r < c->world; ++r) {
+                        if (r == c->rank) continue;
+                        if (int rc2 = xfer_pair(c, st, r, mine, tables + 2 * (size_t)r * n_rec, bytes)) return rc2;
+                    }
+                    return SPH_OK;
+                });
+            if (rc) return rc;
+        }
+        k_shard_body_solve<<<nb, RIGID_THREADS, 0, st>>>(P, c->S, dev_bodies(c), nb, tables, (int)n_rec, c->world);
+        k_enforce_boundary_solid<true><<<blocks_for(P.n_solid, 256), 256, 0, st>>>(P, c->S, nb, dev_bodies(c), nb);
+        *kernels += 2;
+    }
+    k_shard_apply<<<dim3(blocks_for(P.halo_cap, 256), 2), 256, 0, st>>>(P, c->S, /*copy_all=*/1);
+    *kernels += 1;
+    CUDA_TRY(c, cudaGetLastError());
+    rc = shard_exchange(c, st, wide);
+    if (rc) return rc;
+    c->built = false; c->list_valid = false;
+    return SPH_OK;
+}
+
 }  // namespace
 extern "C" {
 
@@ -943,8 +1041,9 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
     if (!ctx) return SPH_E_ARG;
     if (x_lo < 0 || x_hi > ctx->P.gx || ghost_layers < 1 || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
-    // Static solids travel in the records like fluid particles and never change; dynamic solids would need moving
-    // boundary volumes one ghost layer deeper, reactions across a cut and a per-body reduction across ranks.
+    // Static solids travel in the records like fluid particles and never change; dynamic solids need moving boundary
+    // volumes one ghost layer deeper, reactions across a cut and a per-body reduction across ranks: the opt-in
+    // sph_shard_configure_bodies.
     if (!ctx->bodies.empty() || (ctx->P.n_solid > 0 && ctx->has_dynamic_solids))
         return fail(ctx, SPH_E_ARG, kShardStaticOnly);
     if (!ctx->P.uniform_fluid)
@@ -952,10 +1051,20 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
     if (halo_capacity < 1 || 2 * halo_capacity + ctx->P.n > ctx->n_max)
         return fail(ctx, SPH_E_CAPACITY, "capacity: packed particles + 2 * halo_capacity receive slots exceed n_max");
     if (rebalance_every < 0) return SPH_E_ARG;
+    return shard_setup(ctx, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, 0);
+}
+
+}  // extern "C"
+namespace {
+// The part of sph_shard_configure(_bodies) behind the argument checks: the shard buffer (n_body_particles > 0: with
+// the body-particle tables), the device step state and slab mode.
+int shard_setup(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                int32_t rebalance_every, int64_t n_body_particles) {
     const int32_t n_mine = ctx->P.n;
     drop_graphs(ctx);
     if (ctx->shard_buf) { cudaFree(ctx->shard_buf); ctx->shard_buf = nullptr; }
-    ctx->SL = make_shard_layout(halo_capacity, ctx->world);
+    ctx->shard_bodies = false;
+    ctx->SL = make_shard_layout(halo_capacity, ctx->world, n_body_particles);
     CUDA_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->shard_buf), ctx->SL.total));
     CUDA_TRY(ctx, cudaMemset(ctx->shard_buf, 0, ctx->SL.total));
     int32_t sd[SD_INTS] = {0};
@@ -984,6 +1093,47 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
         CUDA_TRY(ctx, cudaEventCreateWithFlags(&ctx->ev_exchanged, cudaEventDisableTiming));
     }
 #endif
+    return SPH_OK;
+}
+
+}  // namespace
+extern "C" {
+
+int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                               int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
+    if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
+    if (x_lo < 0 || x_hi > ctx->P.gx || x_hi - x_lo < ghost_layers + 2)
+        return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
+    if (ghost_layers < 3)
+        return fail(ctx, SPH_E_ARG, "dynamic solids need ghost_layers >= 3: the moving boundary volumes of the second "
+                                    "ghost layer (read by the first layer's densities) sum solids of the third");
+    if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, kShardBodiesWcsph);
+    if (!ctx->P.uniform_fluid)
+        return fail(ctx, SPH_E_ARG, "x-slab sharding needs a single fluid density (uniform fluid masses)");
+    if (halo_capacity < 1 || 2 * halo_capacity + ctx->P.n > ctx->n_max)
+        return fail(ctx, SPH_E_CAPACITY, "capacity: packed particles + 2 * halo_capacity receive slots exceed n_max");
+    if (rebalance_every < 0) return SPH_E_ARG;
+    if (n_bodies > ctx->body_cap) return fail(ctx, SPH_E_CAPACITY, "more rigid bodies than the workspace was sized for");
+    for (int b = 0; b < n_bodies; ++b) {
+        const SphRigidBody &B = bodies[b];
+        if (B.solid_begin < 0 || B.solid_end < B.solid_begin || B.solid_end > ctx->P.n_solid)
+            return fail(ctx, SPH_E_ARG, "rigid body solid-id range out of bounds (pack the whole scene's solid count first)");
+        for (int k = 0; k < 3; ++k)
+            if (!std::isfinite(B.rest_cm[k]))
+                return fail(ctx, SPH_E_ARG, "a sharded body needs its rest centre of mass (computed over the whole scene)");
+    }
+    // on failure the context keeps its previous body table
+    const std::vector<SphRigidBody> old = ctx->bodies;
+    int rc = store_bodies(ctx, bodies, n_bodies);
+    if (rc == SPH_OK)
+        rc = shard_setup(ctx, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, body_particles(ctx->bodies));
+    if (rc) {
+        const std::string why = ctx->err;
+        store_bodies(ctx, old.data(), (int32_t)old.size());
+        ctx->err = why;
+        return rc;
+    }
+    ctx->shard_bodies = true;
     return SPH_OK;
 }
 
@@ -1018,6 +1168,16 @@ int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream) {
     if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_step is the WCSPH step; DFSPH contexts step with sph_shard_dfsph_step");
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (ctx->shard_bodies) {  // always eager: SPH_SHARD_GRAPH does not apply
+        if (ctx->world != ctx->shard_world)
+            return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure_bodies: configure again");
+        for (int s = 0; s < nsteps; ++s) {
+            int rc = shard_bodies_sequence(ctx, st, shard_wide(ctx), &ctx->launches);
+            if (rc) return rc;
+            ctx->shard_sequences += 1;
+        }
+        return SPH_OK;
+    }
     // Un-graphed launches are the DEFAULT here: nothing in a sharded step waits for the host any more, so the launches
     // run ahead of the device, and a graph replay -- whose two branches (exchange || interior forces) must both finish
     // before the next replay may start -- holds back the next step's first kernels, which un-graphed launches queue
@@ -1056,6 +1216,9 @@ int sph_shard_profile_step(SphCtx *ctx, float *ms_out6, void *stream) {
     REQUIRE_SHARD(ctx);
     if (!ms_out6) return SPH_E_ARG;
     if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_profile_step times the WCSPH step");
+    if (ctx->shard_bodies)
+        return fail(ctx, SPH_E_ARG, "sph_shard_profile_step times the static-solid WCSPH step, not the step of a context "
+                                    "configured by sph_shard_configure_bodies");
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaEvent_t ev[8];
@@ -1350,6 +1513,7 @@ int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *st
     REQUIRE_SHARD(ctx);
     if (!io || nsteps < 0 || io->n_fluid < 1) return SPH_E_ARG;
     if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called: WCSPH contexts step with sph_shard_step");
+    if (ctx->shard_bodies) return fail(ctx, SPH_E_ARG, kShardBodiesWcsph);
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     if (ctx->world != ctx->shard_world)
         return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure: configure again");

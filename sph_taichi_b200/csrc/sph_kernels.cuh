@@ -378,17 +378,22 @@ __global__ void k_rank_move(DevParams P, DevArrays S) {
 // Akinci boundary volumes (sph_base.py:91-113).  One WARP per solid particle: the lanes stride
 // over the candidates of the 9 column runs and the partial sums are tree-reduced (a thread per
 // particle left most of the GPU idle: a body has only a few thousand particles).
+// SHARD (sharded steps with dynamic solids, after k_shard_solid_slots): only the solids in the owned layers and the
+// first two ghost layers of each side -- the third one only serves as their neighbours.
+template <bool SHARD = false>
 __global__ void __launch_bounds__(128) k_boundary_volume(DevParams P, DevArrays S, int moving) {
     const int lane = threadIdx.x & 31;
     const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (s >= P.n_solid) return;  // warp-uniform
     const int i = S.solid_slot[s];
+    if (SHARD && i < 0) return;  // not on this rank
     const uint32_t fl = __float_as_uint(S.misc[i].z);
     const bool dyn = (fl & FLAG_DYNAMIC) != 0;
     if (dyn != (moving != 0)) return;
     const float4 pi = S.posm[i];
     int ci, cj, ck;
     cell_of(P, pi.x, pi.y, pi.z, ci, cj, ck);
+    if (SHARD && (ci < S.sd[SD_SX0] - 2 || ci >= S.sd[SD_SX1] + 2)) return;
     ci = min(max(ci, 0), P.gx - 1); cj = min(max(cj, 0), P.gy - 1); ck = min(max(ck, 0), P.gz - 1);
     const int k_lo = max(ck - 1, 0), k_hi = min(ck + 1, P.gz - 1);
     float part = 0.0f;
@@ -592,12 +597,15 @@ struct RigidBodyDev {
 // enforce_boundary_3D(material_solid) restricted to the solid list (cheaper than a full sweep).  reps > 1 with
 // skip_bodies: the fused step applies the n clamps of the reference's body loop to the dynamic solids that belong to NO
 // shape-matched body here (k_rigid does it for the bodies' own particles).
+// SHARD: owned solids only (the slot map of k_shard_solid_slots).
+template <bool SHARD = false>
 __global__ void k_enforce_boundary_solid(DevParams P, DevArrays S, int reps, const RigidBodyDev *skip_bodies, int n_skip) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.n_solid) return;
     for (int b = 0; b < n_skip; ++b)
         if (s >= skip_bodies[b].solid_begin && s < skip_bodies[b].solid_end) return;
     int i = S.solid_slot[s];
+    if (SHARD && (i < S.sd[SD_OWN0] || i >= S.sd[SD_OWN1])) return;  // -1 (not on this rank) or a ghost
     uint32_t fl = __float_as_uint(S.misc[i].z);
     if (!(fl & FLAG_DYNAMIC)) return;
     float4 p = S.posm[i], v = S.veld[i];
@@ -1135,6 +1143,8 @@ struct PackedConst {
     float cp;    // rho0 * m_V of a fluid neighbour
     float cps;   // rho0 * (p_i / rho_i^2 + p_i / rho0^2)  (solid neighbour, WCSPH.py:63)
 };
+// REACT = false (sharded steps): no reaction scatter onto dynamic solids; k_shard_reactions gathers the same terms.
+template <bool REACT = true>
 __device__ __forceinline__ void force_pair_packed(const DevParams &P, const DevArrays &S, ForceAcc &A, int j, float rx,
                                                   float ry, float rz, float r2, const float4 &pj, const float4 &vj,
                                                   const float4 &vi, float dpi, const PackedConst &K) {
@@ -1153,7 +1163,7 @@ __device__ __forceinline__ void force_pair_packed(const DevParams &P, const DevA
         float fx = cp * rx, fy = cp * ry, fz = cp * rz;
         A.prx += fx; A.pry += fy; A.prz += fz;
         float body_rho = -vj.w;
-        if (body_rho < 3.0e38f) {  // dynamic rigid: reaction, WCSPH.py:66-68
+        if (REACT && body_rho < 3.0e38f) {  // dynamic rigid: reaction, WCSPH.py:66-68
             float *a = reinterpret_cast<float *>(S.acc + j);
             float sc = -P.rho0 * rcp_ftz(body_rho);
             atomicAdd(a + 0, fx * sc);
@@ -1208,7 +1218,7 @@ __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevP
     uint32_t fl = __float_as_uint(mi.z);
     if (!(fl & FLAG_FLUID)) {
         // a solid of a send range is staged too, unchanged: k_shard_apply copies the staging back over EVERY record
-        // of the send ranges, and the neighbour's ghost copy comes from it (sharded scenes hold static solids only)
+        // of the send ranges, and the neighbour's ghost copy comes from it (only the static-solid sequence splits)
         if (SHARD && FUSE_ADVECT && split_mode == 1) shard_stage_record(P, S, i, S.posm[i], S.veld[i], S.x0id[i], mi);
         return;
     }
@@ -1249,15 +1259,15 @@ __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevP
             for (int u = 0; u < B; ++u) {
                 float rx = pi.x - pj[u].x, ry = pi.y - pj[u].y, rz = pi.z - pj[u].z;
                 float r2 = rx * rx + ry * ry + rz * rz;
-                force_pair_packed(P, S, A, j[u], rx, ry, rz, r2, pj[u], vj[u], vi, dpi, K);
+                force_pair_packed<!SHARD>(P, S, A, j[u], rx, ry, rz, r2, pj[u], vj[u], vi, dpi, K);
             }
         }
     } else {
         // full scan over the frozen copy (posm may already hold advected neighbours)
         for_all_neighbors<2>(P, S.fpv, S.cell_end, i, pi.x, pi.y, pi.z,
                              [&](int j, float rx, float ry, float rz, float r2, const float4 &pj) {
-                                 force_pair_packed(P, S, A, j, rx, ry, rz, r2, pj, __ldg(S.fpv + 2 * (size_t)j + 1), vi, dpi,
-                                                   K);
+                                 force_pair_packed<!SHARD>(P, S, A, j, rx, ry, rz, r2, pj, __ldg(S.fpv + 2 * (size_t)j + 1),
+                                                           vi, dpi, K);
                              });
     }
     float4 a = make_float4(A.npx + A.prx, A.npy + A.pry, A.npz + A.prz, 0.f);
@@ -1304,6 +1314,202 @@ __global__ void k_advect_solids(DevParams P, DevArrays S) {
     p.x += P.dt * v.x; p.y += P.dt * v.y; p.z += P.dt * v.z;
     S.posm[i] = p;
     S.veld[i] = v;
+}
+
+// =====================================================================================
+// x-slab sharding with dynamic solids (sph_shard_configure_bodies, shard_bodies_sequence)
+// =====================================================================================
+
+// After k_rank_move (which also writes the slots of trash records) and a memset of the map to -1: the slot of every
+// live record's solid id.  A second live record with the same id is a bookkeeping error (SPH_STATUS_SOLID_SLOT).
+__global__ void k_shard_solid_slots(DevParams P, DevArrays S) {
+    const int total = S.cell_end[P.C - 1];
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
+        const int sid = __float_as_int(S.misc[t].w);
+        if (sid < 0 || sid >= P.n_solid) continue;
+        if (atomicMax(S.solid_slot + sid, t) != -1) atomicOr(S.status, SPH_STATUS_SOLID_SLOT);
+    }
+}
+
+__device__ __forceinline__ bool shard_owned_index(const DevArrays &S, int i) {
+    return i >= S.sd[SD_OWN0] && i < S.sd[SD_OWN1];  // false for -1; records of the owned layers are never ghosts
+}
+
+// The reactions of the fluid on the owned dynamic solids as a GATHER (the single engine scatters them from its force
+// pass, which loses the fluid a neighbour owns across a cut), then advect (k_advect_solids).  One warp per solid j
+// walks the 27 cells over the density pass's fpv records: the fluid of the owned layers and the first ghost layer,
+// exactly the records whose fpv and pressure this step's density pass wrote.  Neighbour predicate and pair term are
+// the force pass's, operand for operand (force_pair_packed, solid branch, with i the fluid and j the solid), so only
+// the summation order differs from the single engine's float atomics.
+__global__ void __launch_bounds__(128) k_shard_reactions(DevParams P, DevArrays S) {
+    const int lane = threadIdx.x & 31;
+    const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (s >= P.n_solid) return;  // warp-uniform
+    const int j = S.solid_slot[s];
+    if (!shard_owned_index(S, j)) return;
+    if (!(__float_as_uint(S.misc[j].z) & FLAG_DYNAMIC)) return;
+    const float4 pj = S.fpv[2 * (size_t)j], vj = S.fpv[2 * (size_t)j + 1];
+    const float sc = -P.rho0 * rcp_ftz(-vj.w);  // -rho0 / body density
+    const int d0 = S.sd[SD_DENS0], d1 = S.sd[SD_DENS1];
+    int ci, cj, ck;
+    cell_of(P, pj.x, pj.y, pj.z, ci, cj, ck);
+    ci = min(max(ci, 0), P.gx - 1); cj = min(max(cj, 0), P.gy - 1); ck = min(max(ck, 0), P.gz - 1);
+    const int k_lo = max(ck - 1, 0), k_hi = min(ck + 1, P.gz - 1);
+    float ax = 0.f, ay = 0.f, az = 0.f;
+    for (int dx = -1; dx <= 1; ++dx) {
+        int ni = ci + dx;
+        if (ni < 0 || ni >= P.gx) continue;
+        for (int dy = -1; dy <= 1; ++dy) {
+            int nj = cj + dy;
+            if (nj < 0 || nj >= P.gy) continue;
+            int row = (ni * P.gy + nj) * P.gz;
+            int i0 = max(__ldg(S.cell_end + max(row + k_lo - 1, 0)), d0);
+            int i1 = min(__ldg(S.cell_end + row + k_hi), d1);
+            for (int i = i0 + lane; i < i1; i += 32) {
+                const float4 vi = __ldg(S.fpv + 2 * (size_t)i + 1);
+                if (!(vi.w >= 0.0f)) continue;  // solid (fluid: p / rho^2 >= 0)
+                const float4 pi = __ldg(S.fpv + 2 * (size_t)i);
+                float rx = pi.x - pj.x, ry = pi.y - pj.y, rz = pi.z - pj.z;
+                if (!(exact_r2(rx, ry, rz) < P.h2)) continue;  // the density pass's list predicate, symmetric in i, j
+                float r2 = rx * rx + ry * ry + rz * rz;
+                float wn, G;
+                spline_pair(P, r2, wn, G);
+                const float g1 = G * P.k1_grad;
+                const float cps = P.rho0 * (vi.w + __ldg(&S.misc[i].y) * P.inv_rho0sq);
+                float cp = -(cps * pj.w) * g1;
+                ax += (cp * rx) * sc; ay += (cp * ry) * sc; az += (cp * rz) * sc;
+            }
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        ax += __shfl_xor_sync(0xffffffffu, ax, o);
+        ay += __shfl_xor_sync(0xffffffffu, ay, o);
+        az += __shfl_xor_sync(0xffffffffu, az, o);
+    }
+    if (lane != 0) return;
+    const float4 a = make_float4(P.gx_ + ax, P.gy_ + ay, P.gz_ + az, 0.f);
+    float4 p = S.posm[j], v = S.veld[j];
+    S.acc[j] = a;
+    v.x += P.dt * a.x; v.y += P.dt * a.y; v.z += P.dt * a.z;
+    p.x += P.dt * v.x; p.y += P.dt * v.y; p.z += P.dt * v.z;
+    S.posm[j] = p;
+    S.veld[j] = v;
+}
+
+// Shape matching across ranks.  The body solve must be the single engine's k_rigid bit for bit: its fp32 moments are
+// summed in a fixed order over the solid ids (thread t of a 1024-thread CTA takes s = b0 + t, b0 + t + 1024, ..., then
+// a fixed-order tree), and that rounding moves cm by ~1e-6 of the domain per step even in free fall -- a reduction in
+// any other order or precision drifts from the single engine within a hundred steps and diverges after an impact.
+// So every rank gathers the records of ALL body particles and repeats k_rigid's reduction on them.
+
+// Offset of body b's particles in the gathered table (the bodies' particles in body order, then solid-id order).
+__device__ __forceinline__ int shard_body_offset(const RigidBodyDev *bodies, int b) {
+    int off = 0;
+    for (int k = 0; k < b; ++k) off += bodies[k].solid_end - bodies[k].solid_begin;
+    return off;
+}
+
+// Step 1 (one CTA per body): the clamps the earlier bodies' iterations apply first (k_rigid's pre_clamps), then this
+// rank's entries of the table: rec[2k] = {x, m}, rec[2k + 1] = {x_0, 1} for the owned dynamic body particles, zeros
+// (w = 0: not from this rank) for the others.
+__global__ void k_shard_body_pack(DevParams P, DevArrays S, const RigidBodyDev *bodies, float4 *rec) {
+    const int b = blockIdx.x, pre_clamps = b;
+    const RigidBodyDev *B = bodies + b;
+    const int b0 = B->solid_begin, off = shard_body_offset(bodies, b);
+    for (int s = b0 + threadIdx.x; s < B->solid_end; s += blockDim.x) {
+        float4 *r = rec + 2 * (size_t)(off + s - b0);
+        const int i = S.solid_slot[s];
+        if (!shard_owned_index(S, i) || !(__float_as_uint(S.misc[i].z) & FLAG_DYNAMIC)) {
+            r[0] = make_float4(0.f, 0.f, 0.f, 0.f);
+            r[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+            continue;
+        }
+        float4 p = S.posm[i];
+        if (pre_clamps > 0) {
+            float4 v = S.veld[i];
+            for (int k = 0; k < pre_clamps; ++k) wall_clamp(P, p, v);
+            S.posm[i] = p;
+            S.veld[i] = v;
+        }
+        const float4 x0 = S.x0id[i];
+        r[0] = make_float4(p.x, p.y, p.z, P.m_V0 * S.veld[i].w);
+        r[1] = make_float4(x0.x, x0.y, x0.z, 1.0f);
+    }
+}
+
+// Step 2, after the all-gather of the tables (tables[world][n_rec][2]): one CTA of RIGID_THREADS per body runs k_rigid's
+// mode-2 solve on the gathered records, each taken from the one rank that owns it -- the same operands in the same
+// order, so cm and R equal the single engine's and are bit-identical on every rank.  They go to the body table; the
+// owned body particles move to cm + R q and take this body's and the later bodies' clamps (k_rigid's post_clamps).
+__global__ void __launch_bounds__(RIGID_THREADS) k_shard_body_solve(DevParams P, DevArrays S, RigidBodyDev *bodies,
+                                                                    int n_bodies, const float4 *tables, int n_rec,
+                                                                    int world) {
+    __shared__ float red[32 * 16];
+    __shared__ float s_R[9];
+    const int body = blockIdx.x, post_clamps = n_bodies - body;
+    RigidBodyDev *B = bodies + body;
+    const int b0 = B->solid_begin, b1 = B->solid_end, off = shard_body_offset(bodies, body);
+    const float r0 = B->rest_cm[0], r1 = B->rest_cm[1], r2 = B->rest_cm[2];
+    float acc[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) acc[k] = 0.f;
+    for (int s = b0 + threadIdx.x; s < b1; s += blockDim.x) {
+        const float4 *rec = nullptr;
+        for (int r = 0; r < world && !rec; ++r) {
+            const float4 *t = tables + 2 * ((size_t)r * n_rec + off + (s - b0));
+            if (t[1].w != 0.0f) rec = t;
+        }
+        if (!rec) continue;  // not a dynamic particle (k_rigid skips it too)
+        const float4 p = rec[0], x0 = rec[1];
+        float mass = p.w;
+        float q[3] = {x0.x - r0, x0.y - r1, x0.z - r2};
+        float x[3] = {p.x, p.y, p.z};
+        acc[0] += mass;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            acc[1 + r] += mass * x[r];
+            acc[4 + r] += mass * q[r];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) acc[7 + 3 * r + c] += mass * x[r] * q[c];
+        }
+    }
+    block_reduce<16>(acc, red);
+    const float cmx = acc[1] / acc[0], cmy = acc[2] / acc[0], cmz = acc[3] / acc[0];
+    if (threadIdx.x == 0) {
+        const float cm[3] = {cmx, cmy, cmz};
+        double Ad[9], Rd[9];
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) Ad[3 * r + c] = (double)acc[7 + 3 * r + c] - (double)cm[r] * (double)acc[4 + c];
+        bool ok;
+        polar_rotation_f64(Ad, Rd, ok);
+        if (!ok) atomicOr(S.status, SPH_STATUS_BAD_POLAR);
+        bool all_small = true;
+        float Rf[9];
+        for (int k = 0; k < 9; ++k) { Rf[k] = (float)Rd[k]; if (!(fabsf(Rf[k]) < 1e-6f)) all_small = false; }
+        if (all_small) { for (int k = 0; k < 9; ++k) Rf[k] = (k % 4 == 0) ? 1.0f : 0.0f; }
+        for (int k = 0; k < 9; ++k) { s_R[k] = Rf[k]; B->R[k] = Rf[k]; }
+        B->cm[0] = cmx; B->cm[1] = cmy; B->cm[2] = cmz;
+    }
+    __syncthreads();
+    for (int s = b0 + threadIdx.x; s < b1; s += blockDim.x) {
+        const int i = S.solid_slot[s];
+        if (!shard_owned_index(S, i)) continue;
+        uint32_t fl = __float_as_uint(S.misc[i].z);
+        if (!(fl & FLAG_DYNAMIC)) continue;
+        float4 p = S.posm[i], x0 = S.x0id[i];
+        float q0 = x0.x - r0, q1 = x0.y - r1, q2 = x0.z - r2;
+        float gx = cmx + (s_R[0] * q0 + s_R[1] * q1 + s_R[2] * q2);
+        float gy = cmy + (s_R[3] * q0 + s_R[4] * q1 + s_R[5] * q2);
+        float gz = cmz + (s_R[6] * q0 + s_R[7] * q1 + s_R[8] * q2);
+        p.x += (gx - p.x) * 1.0f; p.y += (gy - p.y) * 1.0f; p.z += (gz - p.z) * 1.0f;
+        if (post_clamps > 0) {
+            float4 v = S.veld[i];
+            for (int r = 0; r < post_clamps; ++r) wall_clamp(P, p, v);
+            S.veld[i] = v;
+        }
+        S.posm[i] = p;
+    }
 }
 
 // Diagnostics: neighbour-list statistics of the last density pass -> out[4] = {max count, particles in

@@ -22,7 +22,18 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
 * Static solids (``RigidBlocks`` / ``RigidBodies`` with ``isDynamic: false``) ride the record exchange like fluid
   particles and never change.  Their boundary volumes depend on solid neighbours that may sit across a cut, so
   ``build_sharded`` computes them once, before the first exchange, over the whole scene exactly as the single engine
-  does (``startup_boundary_volumes``).  Dynamic solids are refused (``STATIC_SOLIDS_ONLY``).
+  does (``startup_boundary_volumes``).
+* Dynamic solids (shape-matched ``RigidBodies`` and advected ``RigidBlocks`` with ``isDynamic: true``) are opt-in,
+  WCSPH only: ``build_sharded(..., dynamic_solids=True)`` configures the engine with ``sph_shard_configure_bodies``.
+  Each rank then keeps 3 ghost layers (a moving solid's boundary volume in the second ghost layer sums solids of the
+  third), gathers the fluid's reactions onto the dynamic solids it owns (fluid owned across a cut included), and
+  solves every body on every rank with the single engine's shape-matching reduction over an all-gather of all body
+  particles' records: cm and R are bit-identical on every rank and equal to the single engine's for the same particle
+  positions (``ShardedSimulation.body_state``).  The bodies' rest centres of mass are computed
+  over the whole scene exactly as the single engine computes them (``startup_rest_cms``).  That step is launched
+  eagerly, without overlap; ``SPH_SHARD_GRAPH`` does not apply.  Without the flag, and for DFSPH in any case, dynamic
+  solids are refused (``STATIC_SOLIDS_ONLY`` / ``DYNAMIC_SOLIDS_WCSPH_ONLY``): the DFSPH pressure sweeps scatter the
+  reactions in every sweep, which would need a reaction exchange per sweep.
 
 ``tests/test_slab_gloo.py`` runs the same library code on the CPU: the host-emulated build of the kernels
 (tests/emu/) with ``GlooTransport`` -- torch.distributed point-to-point over gloo -- in place of NCCL.
@@ -42,14 +53,19 @@ from . import _lib
 
 GHOST_LAYERS = 2
 SEND_LAYERS = GHOST_LAYERS + 2  # one more than the ghost band needs: a cut may move by a layer in any step
+GHOST_LAYERS_BODIES = 3  # dynamic solids: moving boundary volumes of the second ghost layer read the third
+SEND_LAYERS_BODIES = GHOST_LAYERS_BODIES + 2
 RECORD_ARRAYS = 4  # posm, veld, x0id, misc (acc is recomputed every step and not exchanged)
 INFO_KEYS = ("n_live", "owned", "x_lo", "x_hi", "step", "own_begin", "own_end", "sendL_begin", "sendL_end",
              "sendR_begin", "sendR_end", "recv_left", "recv_right", "n_sorted", "status")
 STATUS_OUT_OF_GRID, STATUS_HALO_CAPACITY, STATUS_SHARD_CAPACITY = 1, 4, 8
 STATUS_SHARD_VELOCITY, STATUS_GHOST_ALIGN = 16, 32  # sharded DFSPH (include/sph_b200.h)
+STATUS_SOLID_SLOT = 64  # sharded with dynamic solids: two live records with one solid id
 FLAG_FLUID, FLAG_DYNAMIC, FLAG_GHOST = 1, 2, 4  # misc.z bits of a packed record (csrc/sph_common.cuh)
 STATIC_SOLIDS_ONLY = ("x-slab sharding supports static solids only: dynamic solids (shape-matched bodies, advected "
                       "rigid blocks) are single-GPU in WCSPH and DFSPH")
+DYNAMIC_SOLIDS_WCSPH_ONLY = ("x-slab sharding of dynamic solids is WCSPH only: the DFSPH pressure sweeps scatter the "
+                             "reactions onto the bodies in every sweep, which would need a reaction exchange per sweep")
 
 
 def scene_params(cfg):
@@ -75,8 +91,8 @@ def solid_ids(arrays):
 def field_tensors(arrays, n, m_V0, device):
     """The engine's pack fields of ``n`` particles in the reference's layout (``ParticleSystem.add_particles``:
     x_0 = x, m = density * m_V0); ``arrays["m_V"]`` / ``arrays["solid_id"]`` are used when present."""
-    def t(a, dt):
-        return torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(device)
+    def t(a, dt):  # a copy: on a CPU device, an unpack into the fields must not write through to `arrays`
+        return torch.from_numpy(np.array(a, dtype=dt)).to(device)
 
     dens = t(arrays["density"], np.float32)
     m_V = t(arrays["m_V"], np.float32) if "m_V" in arrays else torch.full((n,), m_V0, dtype=torch.float32, device=device)
@@ -120,6 +136,39 @@ def startup_boundary_volumes(cfg, arrays, device):
     by_sid[got_sid[s]] = got_mV[s]
     out[sid >= 0] = by_sid[sid[sid >= 0]]
     return out
+
+
+def dynamic_bodies(cfg, arrays):
+    """The shape-matched bodies as the single engine registers them (``ParticleSystem._prepare_solids``): every
+    dynamic ``RigidBodies`` object in object-id order, with the range of its global solid ids (``solid_ids``).
+    Returns [(object_id, solid_begin, solid_end)]."""
+    sid, oid = np.asarray(arrays["solid_id"]), np.asarray(arrays["object_id"])
+    out = []
+    for b in sorted((cfg.get_rigid_bodies() or []), key=lambda b_: b_["objectId"]):
+        if not b["isDynamic"]:
+            continue
+        ids = sid[(oid == b["objectId"]) & (sid >= 0)]
+        if ids.size:
+            out.append((int(b["objectId"]), int(ids.min()), int(ids.max()) + 1))
+    return out
+
+
+def startup_rest_cms(cfg, arrays, bodies, device):
+    """Each body's rest centre of mass as ``SPHBase.compute_rigid_rest_cm`` computes it at start-up: the same kernel
+    on the same packed scene (the sum runs in solid-id order), hence bit-identical to the single engine's."""
+    from . import engine as _engine
+    n = len(arrays["material"])
+    sid = np.asarray(arrays["solid_id"])
+    n_solid = int((sid >= 0).sum())
+    m_V0 = float(np.float32(0.8 * (2 * cfg.get_cfg("particleRadius")) ** 3))
+    eng = _engine.Engine(scene_params(cfg), n_max=n, n_solid=n_solid, n_bodies=len(bodies), device=device)
+    try:
+        eng.pack(field_tensors(arrays, n, m_V0, device), n, n_solid, True)
+        eng.set_rigid_bodies([(o, b0, b1, [np.nan] * 3) for o, b0, b1 in bodies])
+        eng.neighbor_build()
+        return [eng.compute_com(b).cpu().numpy().astype(np.float32) for b in range(len(bodies))]
+    finally:
+        eng.close()
 
 
 def plan_slabs(layer_counts, world, min_width=SEND_LAYERS + 1):
@@ -200,10 +249,12 @@ class ShardedSimulation:
     """This rank's share of a sharded scene: a CUDA engine in slab mode + the library's halo exchange."""
 
     def __init__(self, cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, uniform_hint, group=None,
-                 rebalance_every=8, transport=None, n_fluid=None, n_solid=0):
+                 rebalance_every=8, transport=None, n_fluid=None, n_solid=0, bodies=None):
         """``mine``: this rank's initial particles (numpy arrays in the reference's field layout); with solids also
         ``solid_id`` (global ids, ``solid_ids``) and ``m_V`` (start-up boundary volumes, ``startup_boundary_volumes``).
-        ``n_solid``: the solid count of the WHOLE scene (sizes the solid-id slot map)."""
+        ``n_solid``: the solid count of the WHOLE scene (sizes the solid-id slot map).  ``bodies`` (dynamic solids,
+        WCSPH): [(object_id, solid_begin, solid_end, rest_cm)] of the whole scene (``dynamic_bodies``,
+        ``startup_rest_cms``), an empty list for advected rigid blocks only; None refuses dynamic solids."""
         from . import engine as _engine
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dfsph = cfg.get_cfg("simulationMethod") == 4
@@ -217,8 +268,11 @@ class ShardedSimulation:
         self.grid_num = np.ceil(ds / self.h).astype(int)
         self.m_V0 = float(np.float32(0.8 * (2 * radius) ** 3))
         self.n_cap, self.halo_cap, self.n_solid = int(n_cap), int(halo_cap), int(n_solid)
-        self.eng = _engine.Engine(scene_params(cfg), n_max=self.n_cap, n_solid=self.n_solid, n_bodies=0,
-                                  device=self.device)
+        self.bodies = None if bodies is None else list(bodies)
+        if self.bodies is not None and self.dfsph:
+            raise NotImplementedError(DYNAMIC_SOLIDS_WCSPH_ONLY)
+        self.eng = _engine.Engine(scene_params(cfg), n_max=self.n_cap, n_solid=self.n_solid,
+                                  n_bodies=len(self.bodies or []), device=self.device)
         e = self.eng
         self._load(mine, n_mine, uniform_hint)
         self.last_iterations_v = self.last_iterations = 0
@@ -244,20 +298,30 @@ class ShardedSimulation:
         else:
             e._check(e.lib.sph_comm_set_transport(e.ctx, None, 0, 1), "sph_comm_set_transport")
         lo, hi = self.slabs0[rank]
-        e._check(e.lib.sph_shard_configure(e.ctx, lo, hi, GHOST_LAYERS, self.halo_cap, int(rebalance_every)),
-                 "sph_shard_configure")
+        if self.bodies is None:
+            e._check(e.lib.sph_shard_configure(e.ctx, lo, hi, GHOST_LAYERS, self.halo_cap, int(rebalance_every)),
+                     "sph_shard_configure")
+        else:
+            table = (_lib.SphRigidBody * max(1, len(self.bodies)))()
+            for i, (oid, b0, b1, rest_cm) in enumerate(self.bodies):
+                table[i].object_id, table[i].solid_begin, table[i].solid_end = int(oid), int(b0), int(b1)
+                table[i].rest_cm = (C.c_float * 3)(*[float(v) for v in rest_cm])
+            e._check(e.lib.sph_shard_configure_bodies(e.ctx, lo, hi, GHOST_LAYERS_BODIES, self.halo_cap,
+                                                      int(rebalance_every), table, len(self.bodies)),
+                     "sph_shard_configure_bodies")
         e._check(e.lib.sph_shard_begin(e.ctx, e._stream()), "sph_shard_begin")
         self.steps_done = 0
 
     def _load(self, arrays, n, uniform_hint):
         """Pack this rank's initial particles (numpy arrays in the reference's field layout)."""
         solid = np.asarray(arrays["material"]) != 1
-        if bool((solid & (np.asarray(arrays["is_dynamic"]) != 0)).any()):
+        dynamic = self.bodies is not None
+        if not dynamic and bool((solid & (np.asarray(arrays["is_dynamic"]) != 0)).any()):
             raise NotImplementedError(STATIC_SOLIDS_ONLY)
         if solid.any() and ("solid_id" not in arrays or "m_V" not in arrays):
             raise ValueError("solid particles need their global solid_id and start-up m_V (see build_sharded)")
         f = field_tensors(arrays, n, self.m_V0, self.device)
-        self.eng.pack(f, n, self.n_solid, False, uniform_hint=uniform_hint)
+        self.eng.pack(f, n, self.n_solid, dynamic, uniform_hint=uniform_hint)
         self.synchronize()  # the temporaries above may be freed now
 
     # ---- stepping --------------------------------------------------------------------------------------
@@ -274,6 +338,12 @@ class ShardedSimulation:
         else:
             e._check(e.lib.sph_shard_step(e.ctx, int(n), e._stream()), "sph_shard_step")
         self.steps_done += int(n)
+
+    def body_state(self, b):
+        """(cm [3], R [3, 3]) of body ``b`` (index into ``bodies``) after the last step, as numpy arrays; the same
+        bits on every rank."""
+        R, cm = self.eng.rigid_state(b)
+        return cm, R
 
     def transport_stats(self):
         """(transport groups issued, bytes this rank sent in them) since the engine was created."""
@@ -308,6 +378,8 @@ class ShardedSimulation:
         if st & STATUS_SHARD_VELOCITY:
             raise RuntimeError(f"rank {self.rank}: a particle moved a whole cell layer in x within one step "
                                f"(|v_x| * dt >= h); the record exchange may have lost it -- reduce timeStepSize")
+        if st & STATUS_SOLID_SLOT:
+            raise RuntimeError(f"rank {self.rank}: two live records carry the same solid id (status {st})")
         if st & STATUS_GHOST_ALIGN:
             raise RuntimeError(f"rank {self.rank}: a neighbour's boundary layers and this rank's ghost layers differ "
                                f"(status {st})")
@@ -362,9 +434,11 @@ class ShardedSimulation:
 
 
 def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1.2, rebalance_every=8, slabs=None,
-                  transport=None):
+                  transport=None, dynamic_solids=False):
     """Assemble the scene on every rank, plan the slabs from the initial layer histogram and load this rank's
-    share into a CUDA engine.  Returns (ShardedSimulation, n_total)."""
+    share into a CUDA engine.  ``dynamic_solids=True`` opts in to sharding WCSPH scenes with dynamic solids
+    (3 ghost layers, reactions gathered across cuts, bodies solved on every rank from an all-gather of their particles).
+    Returns (ShardedSimulation, n_total)."""
     from .config_builder import SimConfig
     from .scene import assemble_particles
 
@@ -376,15 +450,23 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     gx = int(np.ceil(ds / h).astype(int)[0])
     lay = layer_of(arrays["x"], h)
     hist = np.bincount(lay, minlength=gx)[:gx]
+    send_layers = SEND_LAYERS_BODIES if dynamic_solids else SEND_LAYERS
+    ghost_layers = GHOST_LAYERS_BODIES if dynamic_solids else GHOST_LAYERS
+    if dynamic_solids and cfg.get_cfg("simulationMethod") == 4:
+        raise NotImplementedError(DYNAMIC_SOLIDS_WCSPH_ONLY)
     if slabs is None:
-        slabs = plan_slabs(hist, world)
+        slabs = plan_slabs(hist, world, min_width=send_layers + 1)
     fluid = arrays["material"] == 1
-    if bool((~fluid & (arrays["is_dynamic"] != 0)).any()):
+    if not dynamic_solids and bool((~fluid & (arrays["is_dynamic"] != 0)).any()):
         raise NotImplementedError(STATIC_SOLIDS_ONLY)
     n_solid = int((~fluid).sum())
+    bodies = None
     if n_solid:
         arrays["solid_id"] = solid_ids(arrays)
         arrays["m_V"] = startup_boundary_volumes(cfg, arrays, device)
+    if dynamic_solids:
+        table = dynamic_bodies(cfg, arrays) if n_solid else []
+        bodies = [t + (cm,) for t, cm in zip(table, startup_rest_cms(cfg, arrays, table, device))] if table else []
     lo, hi = slabs[rank]
     mine, n_mine = select_owned(arrays, h, lo, hi)
     # one decision for the whole scene (a rank may start empty), the single engine's: all FLUID particles share m
@@ -394,12 +476,12 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     uniform = bool(m_fluid.size and (m_fluid == m_fluid[0]).all())
     hint = (uniform, float(m_fluid[0]) if m_fluid.size else 0.0, float(m_V0))
     # the fullest layer bounds every layer the front may reach later: SEND_LAYERS of them per side and direction
-    halo_cap = int(SEND_LAYERS * int(hist.max()) * capacity_factor) + 1024
-    ghost_est = 2 * GHOST_LAYERS * int(hist.max())
+    halo_cap = int(send_layers * int(hist.max()) * capacity_factor) + 1024
+    ghost_est = 2 * ghost_layers * int(hist.max())
     n_cap = int((n_mine + ghost_est) * capacity_factor) + 4 * halo_cap + 1024  # live + trash + 2 receive regions
     sim = ShardedSimulation(cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, hint, group=group,
                             rebalance_every=rebalance_every, transport=transport, n_fluid=int(fluid.sum()),
-                            n_solid=n_solid)
+                            n_solid=n_solid, bodies=bodies)
     return sim, counts["total"]
 
 
@@ -446,10 +528,12 @@ def gather_owned(sim, dst=0):
     return split(torch.cat([b[:c] for b, c in zip(bufs, counts)], dim=0))
 
 
-def compare_with_single(gathered, ps, d):
+def compare_with_single(gathered, ps, d, bodies=None):
     """Rank 0: the gathered sharded state against a ParticleSystem that ran the same steps on ONE GPU, particles
     matched by (object_id, x_0).  With solids in the scene it also reports whether every static solid is still
-    exactly at x_0 and the largest relative difference of the static solids' m_V from the single engine's."""
+    exactly at x_0 and the largest relative difference of the static solids' m_V from the single engine's.  With
+    dynamic solids: the largest distance of the fluid and of the dynamic solids alone (over d); with ``bodies``
+    ({object_id: (cm, R)} of the sharded run) per body |cm - cm_single| / d and max |R - R_single|."""
     X, V, X0, OID, MV, FL = gathered
     ps._pull()
     n = int(ps.particle_num[None])
@@ -469,6 +553,21 @@ def compare_with_single(gathered, ps, d):
                 out = {"static_solids": int(static.sum().item()),
                        "static_solids_at_x0": bool(torch.equal(X[ks][static], X0[ks][static])),
                        "max_rel_dm_V_static": float(((a - b).abs() / b.abs()).max().item())}
+            dyn = ((FL[ks] & (FLAG_FLUID | FLAG_DYNAMIC)) == FLAG_DYNAMIC)
+            if bool(dyn.any()):
+                fl = (FL[ks] & FLAG_FLUID) != 0
+                dist_ = (X[ks] - rx[kr]).abs().max(dim=1).values / d
+                out["dynamic_solids"] = int(dyn.sum().item())
+                out["max_dx_over_d_dynamic_solids"] = float(dist_[dyn].max().item())
+                out["max_dx_over_d_fluid"] = float(dist_[fl].max().item()) if bool(fl.any()) else 0.0
+    if bodies:
+        rows = []
+        for oid in sorted(bodies):
+            cm, R = (np.asarray(t, np.float64) for t in bodies[oid])
+            R1, cm1 = ps._engine.rigid_state(ps._body_index[oid])
+            rows.append({"object_id": int(oid), "dcm_over_d": float(np.abs(cm - cm1).max() / d),
+                         "max_dR": float(np.abs(R - R1).max())})
+        out["bodies"] = rows
     return dict({"same_particle_set": bool(same), "max_dx_over_d": dx, "max_dv": dv, "particles": int(X0.shape[0])},
                 **out)
 

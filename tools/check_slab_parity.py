@@ -13,6 +13,13 @@ static solid is still exactly at x_0 with the single engine's start-up boundary 
 with the single engine's, checks that every rank reported bit-identical counts and average errors in every step, and
 that after the last step's ghost alignment each ghost record holds the x_0 of the neighbour's boundary record at the
 same position.
+
+--dynamic-body / --dynamic-block add dynamic solids (WCSPH, build_sharded(dynamic_solids=True)): a shape-matched cube
+(tests/golden/cube.obj) straddling the fluid's x fraction 1/world (1/2 on one rank) -- the initial cut of a balanced
+start -- and resting on the fluid surface, and an advected dynamic rigid block on the surface at 3/4 of the fluid.  The tool then also reports whether
+every body's cm and R were bit-identical on every rank after every step, whether the fluid's reactions acted (every
+dynamic object's mean velocity left free fall, in both engines), and the per-body cm / R differences; "ok" then also
+requires max_dv < 1e-2 and per-body |dcm| / d and max |dR| below 1e-3.
 """
 import argparse
 import json
@@ -47,6 +54,37 @@ def static_block_scene(c, d):
     return sc
 
 
+def add_dynamic_solids(sc, c, d, world, body, block):
+    """The dynamic solids of --dynamic-body / --dynamic-block on top of the dam break of ``c`` particles (start 0.06)."""
+    x0, top, z0 = 0.06, 0.06 + c[1] * d, 0.06
+    side = 4.5 * d
+    if body:
+        cut = x0 + c[0] * d / max(world, 2)  # world 1: the middle
+        sc.setdefault("RigidBodies", []).append({
+            "objectId": 2, "geometryFile": os.path.join(ROOT, "tests", "golden", "cube.obj"),
+            "translation": [cut - side / 2, top + 0.25 * d, z0 + (c[2] * d - side) / 2], "rotationAxis": [0, 1, 0],
+            "rotationAngle": 0, "scale": [side] * 3, "velocity": [0.0, 0.0, 0.0], "density": 800.0,
+            "color": [255, 255, 255], "isDynamic": True})
+    if block:
+        bx = x0 + 0.75 * c[0] * d
+        sc.setdefault("RigidBlocks", []).append({
+            "objectId": 3, "start": [bx, top, z0 + d], "end": [bx + 2.5 * d, top + 2.5 * d, z0 + 3.5 * d],
+            "translation": [0.0, 0.0, 0.0], "scale": [1, 1, 1], "velocity": [0.0, 0.0, 0.0], "density": 600.0,
+            "color": [255, 0, 0], "isDynamic": True})
+    return sc
+
+
+def dynamic_velocities(V, OID, FL, g_y, t):
+    """{object_id: (mean v_y, deviation from free fall)} of the dynamic solids (objects start at rest)."""
+    out = {}
+    dyn = (FL & 3) == 2
+    for oid in sorted(set(OID[dyn].tolist())):
+        m = dyn & (OID == oid)
+        vy = float(V[m][:, 1].double().mean())
+        out[int(oid)] = (vy, abs(vy - g_y * t))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--counts", type=int, nargs=3, default=[64, 24, 24])
@@ -57,6 +95,8 @@ def main():
     ap.add_argument("--dfsph", action="store_true", help="DFSPH instead of WCSPH (simulationMethod 4, dt = 4e-3)")
     ap.add_argument("--static-block", action="store_true",
                     help="the fluid rests on a static rigid block that straddles every cut (static_block_scene)")
+    ap.add_argument("--dynamic-body", action="store_true", help="a shape-matched cube across the initial cut (WCSPH)")
+    ap.add_argument("--dynamic-block", action="store_true", help="an advected dynamic rigid block (WCSPH)")
     ap.add_argument("--scene", default=None, choices=sorted(scene.NAMED_SCENES),
                     help="a named scene as it is (--counts, --vx and --static-block do not apply; a DFSPH scene needs "
                          "--dfsph for the iteration-count comparison)")
@@ -83,6 +123,11 @@ def main():
         sc = static_block_scene(c, d)
     else:
         sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12], start=[0.06] * 3)
+    dynamic = a.dynamic_body or a.dynamic_block
+    if dynamic and not a.scene:
+        sc = add_dynamic_solids(sc, c, d, world, a.dynamic_body, a.dynamic_block)
+    if a.scene and any(b.get("isDynamic") for b in sc.get("RigidBodies", []) + sc.get("RigidBlocks", [])):
+        dynamic = True
     if not a.scene:
         sc["FluidBlocks"][0]["velocity"] = [a.vx, 0.0, 0.0]
     if a.dfsph and sc["Configuration"]["simulationMethod"] != 4:
@@ -100,7 +145,7 @@ def main():
         cuts = [cuts[0]] + [c_ + a.skew for c_ in cuts[1:-1]] + [cuts[-1]]
         slabs = [(cuts[r], cuts[r + 1]) for r in range(world)]
     sim, n_total = slab.build_sharded(sc, rank, world, dev, rebalance_every=a.rebalance_every, slabs=slabs,
-                                      transport=transport)
+                                      transport=transport, dynamic_solids=dynamic)
     first = sim.info()
     trace = []
     if a.soak:
@@ -115,6 +160,11 @@ def main():
         for _ in range(a.steps):  # one step per call: the iteration counts of every step
             sim.step(1)
             trace.append((sim.last_iterations_v, sim.last_iterations, sim.last_avg_err_v.hex(), sim.last_avg_err.hex()))
+    elif dynamic:
+        for _ in range(a.steps):  # one step per call: the body states of every step
+            sim.step(1)
+            trace.append([[c_.tobytes().hex(), R_.tobytes().hex()] for c_, R_ in
+                          (sim.body_state(b) for b in range(len(sim.bodies)))])
     else:
         sim.step(a.steps)
     last = sim.info()
@@ -129,6 +179,10 @@ def main():
         meta["x0_ghost_right"] = x0[last["own_end"]:last["n_live"]].tolist()
         meta["x0_owned"] = x0[last["own_begin"]:last["own_end"]].tolist()
         meta["transport"] = sim.transport_stats()
+    if dynamic:
+        meta["transport"] = sim.transport_stats()
+        meta["halo_cap"] = sim.halo_cap
+        meta["body_particles"] = sum(b1 - b0 for _, b0, b1, _cm in sim.bodies)
     metas = [None] * world
     if world > 1:
         dist.all_gather_object(metas, meta)
@@ -145,7 +199,11 @@ def main():
                 single_counts.append([s.last_iterations_v, s.last_iterations])
         else:
             s.step(a.steps)
-        cmp_ = slab.compare_with_single(gathered, ps, d)
+        bodies = None
+        if dynamic:
+            bodies = {oid: sim.body_state(b) for b, (oid, *_rest) in enumerate(sim.bodies)}
+        cmp_ = slab.compare_with_single(gathered, ps, d, bodies=bodies)
+        X0, OID0 = gathered[2], gathered[3]
         migrated = any(m["owned"][0] != m["owned"][1] for m in metas)
         moved = any(tuple(m["slab0"]) != tuple(m["slab1"]) for m in metas)
         ok = cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < 1e-3 and cmp_["max_dv"] < 1e-2 and slab.static_solids_ok(cmp_)
@@ -153,6 +211,9 @@ def main():
         if bool(solid.any()):  # [first, last + 1) cell layer the solids occupy
             lay = slab.layer_of(ps._t["x"][:n_total][solid].cpu().numpy(), 2 * d)
             cmp_["solid_layers"] = [int(lay.min()), int(lay.max()) + 1]
+        if a.dynamic_body and not a.scene:  # [first, last + 1) cell layer the cube occupies at the start
+            lay = slab.layer_of(np.asarray(X0[OID0 == 2].cpu().numpy()), 2 * d)
+            cmp_["body_layers"] = [int(lay.min()), int(lay.max()) + 1]
         if a.dfsph:
             counts = [list(t[:2]) for t in metas[0]["trace"]]
             same_on_ranks = all([list(t) for t in m["trace"]] == [list(t) for t in metas[0]["trace"]] for m in metas)
@@ -171,6 +232,25 @@ def main():
                         bit_identical_across_ranks=same_on_ranks, ghosts_aligned=aligned,
                         transport_groups=[m["transport"][0] for m in metas],
                         transport_bytes=[m["transport"][1] for m in metas])
+        if dynamic:
+            same_on_ranks = all(m["trace"] == metas[0]["trace"] for m in metas)
+            g_y, t = float(sc["Configuration"]["gravitation"][1]), a.steps * float(sc["Configuration"]["timeStepSize"])
+            X, V, X0, OID, MV, FL = gathered
+            vs = dynamic_velocities(V, OID, FL, g_y, t)
+            ps._pull()
+            n_ = int(ps.particle_num[None])
+            fl1 = (ps._t["material"][:n_] != 1).int() * 2 * (ps._t["is_dynamic"][:n_] != 0).int()
+            v1 = dynamic_velocities(ps._t["v"][:n_], ps._t["object_id"][:n_], fl1, g_y, t)
+            acted = bool(vs) and all(vs[o][1] > 1e-3 and v1[o][1] > 1e-3 for o in vs)
+            bodies_ok = all(b["dcm_over_d"] < 1e-3 and b["max_dR"] < 1e-3 for b in cmp_.get("bodies", []))
+            ok = (cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < 1e-3 and cmp_["max_dv"] < 1e-2
+                  and same_on_ranks and bodies_ok and slab.static_solids_ok(cmp_))
+            cmp_ = dict(cmp_, bodies_bit_identical_across_ranks=same_on_ranks, reactions_acted=acted,
+                        dynamic_vy_sharded={str(k): v[0] for k, v in vs.items()},
+                        dynamic_vy_single={str(k): v[0] for k, v in v1.items()}, free_fall_vy=g_y * t,
+                        n_bodies=len(sim.bodies), transport_groups=[m["transport"][0] for m in metas],
+                        transport_bytes=[m["transport"][1] for m in metas], halo_cap=[m["halo_cap"] for m in metas],
+                        body_particles=metas[0]["body_particles"])
         if a.soak:
             X, V = gathered[:2]
             ps._pull()
