@@ -284,6 +284,27 @@ int sph_halo_exchange(SphCtx *ctx, void *stream);
  * own_end, sendL_begin, sendL_end, sendR_begin, sendR_end, recv_left, recv_right, n_sorted, status,
  * 0}; out_sent (may be NULL) = halo records sent so far */
 int sph_shard_info(SphCtx *ctx, int32_t *out16, uint64_t *out_sent, void *stream);
+/* Output of a sharded run: x and v of ONE object gathered on rank 0 (ParticleSystem.dump, particle_system.py:409-418).
+ * Collective over the sharded context's ranks, synchronising; call it on every rank at the same point between steps,
+ * with the same object_id.  x, v: [capacity, 3] float32 device buffers (the layout of sph_unpack_xv).
+ *   - Each rank takes its owned records -- the index range [own_begin, own_end) of the last sort without the ghost
+ *     flag, a partition of the particles -- whose object id is object_id, and compacts their x and v on the device
+ *     in its sorted order (deterministic, no atomics).
+ *   - One transport group: every rank sends {capacity, rows, status word} (16 bytes) to every other rank, so every rank
+ *     evaluates the same check: if rank 0's capacity is below the total rows, or any rank's capacity below its own
+ *     rows, EVERY rank returns SPH_E_CAPACITY (the message names the capacity) and no rank transfers anything.
+ *   - A second group (only if a rank other than 0 holds rows): each rank r > 0 with rows sends them to rank 0, which
+ *     receives them behind the rows of ranks 0 .. r - 1; rank 0's own rows are at row 0.
+ * On rank 0 *rows_out is the total and x / v hold every rank's rows in rank order; slabs are contiguous x-layer
+ * ranges in rank order and the cell flattening is x-major, so that is the global cell order of the last sort.  On
+ * the other ranks *rows_out is their own row count and x / v hold their own rows.  *status_out is the OR of every
+ * rank's status word (sph_shard_info's), the same on every rank, also when SPH_E_CAPACITY is returned.
+ * sph_shard_transport_stats counts the bytes like any other group: this rank sends (world - 1) * 16 bytes of headers,
+ * plus, on ranks other than rank 0, 24 bytes (x and v, 3 float32 each) per row it holds.  Launches nothing into
+ * sph_shard_step's graphs; works on WCSPH, DFSPH and sph_shard_configure_bodies contexts.  Single-GPU contexts are
+ * refused (they have sph_unpack_xv); capacity < 0 or a null pointer returns SPH_E_ARG. */
+int sph_shard_dump(SphCtx *ctx, int32_t object_id, float *x, float *v, int64_t capacity, int64_t *rows_out,
+                   uint32_t *status_out, void *stream);
 /* ONE un-graphed sharded step with CUDA events between its stages; ms_out6 = {plan + sort + info, boundary
  * densities, boundary forces (-> staging), interior densities, apply + interior forces (+ waiting for the exchange,
  * if it is not hidden), the exchange alone on the communication stream}; synchronises */

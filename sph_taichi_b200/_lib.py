@@ -27,7 +27,7 @@ ABI_SYMBOLS = [
     "sph_launch_count", "sph_profile_step", "sph_timer_name", "sph_state_offsets", "sph_set_dfsph", "sph_dfsph_op", "sph_dfsph_solve", "sph_dfsph_step",
     "sph_comm_unique_id", "sph_comm_init_nccl", "sph_comm_set_transport", "sph_shard_configure", "sph_shard_begin",
     "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step", "sph_shard_dfsph_step",
-    "sph_shard_transport_stats", "sph_shard_configure_bodies",
+    "sph_shard_transport_stats", "sph_shard_configure_bodies", "sph_shard_dump",
 ]
 
 
@@ -161,6 +161,7 @@ def load():
         "sph_shard_profile_step": (C.c_int, [vp, C.POINTER(C.c_float), vp]),
         "sph_shard_dfsph_step": (C.c_int, [vp, i32, C.POINTER(SphDfsphStep), vp]),
         "sph_shard_transport_stats": (C.c_int, [vp, C.POINTER(u64)]),
+        "sph_shard_dump": (C.c_int, [vp, i32, vp, vp, i64, C.POINTER(i64), C.POINTER(C.c_uint32), vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

@@ -200,6 +200,10 @@ struct SphCtx {
     int shard_world = 1;  // world size the shard buffer's per-rank error partials were sized for
     bool shard_bodies = false;  // configured by sph_shard_configure_bodies: steps with shard_bodies_sequence
     uint64_t xfer_groups = 0, xfer_bytes = 0;  // transport groups issued from the host, and the bytes this rank sent
+    // sph_shard_dump's device scratch (library-owned, grown on demand): the header sent, the headers received, the
+    // tile counts
+    char *dump_buf = nullptr;
+    uint64_t dump_bytes = 0;
 };
 
 namespace {
@@ -534,6 +538,7 @@ int sph_destroy(SphCtx *ctx) {
     if (ctx->ev_exchanged) cudaEventDestroy(ctx->ev_exchanged);
 #endif
     if (ctx->shard_buf) cudaFree(ctx->shard_buf);
+    if (ctx->dump_buf) cudaFree(ctx->dump_buf);
     delete ctx;
     return SPH_OK;
 }
@@ -814,6 +819,19 @@ int xfer_pair(SphCtx *c, cudaStream_t st, int peer, const void *sp, void *rp, ui
     TRANSPORT_OP(st, t.send(t.user, sp, bytes, peer, st));
     TRANSPORT_OP(st, t.recv(t.user, rp, bytes, peer, st));
     c->xfer_bytes += bytes;
+    return SPH_OK;
+}
+
+// One-way messages inside a transport group (sph_shard_dump's gather); a send counts its bytes.
+int xfer_send(SphCtx *c, cudaStream_t st, int peer, const void *sp, uint64_t bytes) {
+    const SphTransport t = c->transport;
+    TRANSPORT_OP(st, t.send(t.user, sp, bytes, peer, st));
+    c->xfer_bytes += bytes;
+    return SPH_OK;
+}
+int xfer_recv(SphCtx *c, cudaStream_t st, int peer, void *rp, uint64_t bytes) {
+    const SphTransport t = c->transport;
+    TRANSPORT_OP(st, t.recv(t.user, rp, bytes, peer, st));
     return SPH_OK;
 }
 
@@ -1209,6 +1227,115 @@ int sph_shard_info(SphCtx *ctx, int32_t *out16, uint64_t *out_sent, void *stream
     for (int k = 0; k < 14; ++k) out16[k] = sd[k];
     out16[14] = (int32_t)status; out16[15] = 0;
     if (out_sent) *out_sent = ((uint64_t)(uint32_t)sd[SD_SENT_HI] << 32) | (uint32_t)sd[SD_SENT_LO];
+    return SPH_OK;
+}
+
+// What every rank tells every other rank before the gather of sph_shard_dump (16 bytes)
+struct DumpHeader {
+    int64_t capacity;
+    int32_t rows;
+    uint32_t status;
+};
+static_assert(sizeof(DumpHeader) == 16, "the dump header travels as 16 bytes");
+
+int sph_shard_dump(SphCtx *ctx, int32_t object_id, float *x, float *v, int64_t capacity, int64_t *rows_out,
+                   uint32_t *status_out, void *stream) {
+    REQUIRE_SHARD(ctx);
+    if (!x || !v || !rows_out || !status_out || capacity < 0)
+        return fail(ctx, SPH_E_ARG, "sph_shard_dump: x, v, rows_out and status_out must be non-null and capacity >= 0");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int world = ctx->world, rank = ctx->rank;
+    // the owned range of the last sort sizes the grid
+    int32_t own[2] = {0, 0};
+    CUDA_TRY(ctx, cudaMemcpyAsync(own, ctx->S.sd + SD_OWN0, sizeof(own), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    const int n_tiles = (int)((std::max(own[1] - own[0], 0) + DUMP_TILE - 1) / DUMP_TILE);
+    const uint64_t off_recv = 256, off_counts = off_recv + align_up((uint64_t)world * sizeof(DumpHeader), 256);
+    const uint64_t need = off_counts + (uint64_t)(n_tiles + 1) * 4;
+    if (need > ctx->dump_bytes) {
+        if (ctx->dump_buf) cudaFree(ctx->dump_buf);
+        ctx->dump_buf = nullptr; ctx->dump_bytes = 0;
+        CUDA_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->dump_buf), need));
+        ctx->dump_bytes = need;
+    }
+    DumpHeader *hdr_send = reinterpret_cast<DumpHeader *>(ctx->dump_buf);
+    DumpHeader *hdr_recv = reinterpret_cast<DumpHeader *>(ctx->dump_buf + off_recv);
+    int32_t *counts = reinterpret_cast<int32_t *>(ctx->dump_buf + off_counts);
+    if (n_tiles > 0) {
+        k_dump_count<<<n_tiles, DUMP_THREADS, 0, st>>>(ctx->S, own[0], own[1], object_id, counts);
+        k_dump_scan<<<1, DUMP_THREADS, 0, st>>>(counts, n_tiles);
+        ctx->launches += 2;
+        CUDA_TRY(ctx, cudaGetLastError());
+    } else {
+        CUDA_TRY(ctx, cudaMemsetAsync(counts, 0, 4, st));
+    }
+    DumpHeader mine{capacity, 0, 0u};
+    CUDA_TRY(ctx, cudaMemcpyAsync(&mine.rows, counts + n_tiles, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(&mine.status, ctx->S.status, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    // group 1: {capacity, rows, status} to every other rank, so that every rank takes the same decision below
+    std::vector<DumpHeader> all((size_t)world, DumpHeader{0, 0, 0u});
+    if (world > 1) {
+        CUDA_TRY(ctx, cudaMemcpyAsync(hdr_send, &mine, sizeof(mine), cudaMemcpyHostToDevice, st));
+        int rc = transport_group(
+            ctx, st, [](int, int) { return SPH_OK; },
+            [&] {
+                for (int r = 0; r < world; ++r) {
+                    if (r == rank) continue;
+                    if (int rc2 = xfer_pair(ctx, st, r, hdr_send, hdr_recv + r, sizeof(DumpHeader))) return rc2;
+                }
+                return SPH_OK;
+            });
+        if (rc) return rc;
+        CUDA_TRY(ctx, cudaMemcpyAsync(all.data(), hdr_recv, (size_t)world * sizeof(DumpHeader), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    }
+    all[(size_t)rank] = mine;
+    int64_t total = 0;
+    uint32_t status = 0u;
+    for (const DumpHeader &h : all) { total += h.rows; status |= h.status; }
+    *rows_out = rank == 0 ? total : mine.rows;
+    *status_out = status;
+    // the same check, in rank order, on every rank: all of them return here, or none does
+    if (all[0].capacity < total)
+        return fail(ctx, SPH_E_CAPACITY, "sph_shard_dump: capacity: rank 0 gathers " + std::to_string(total) + " rows of object " +
+                                         std::to_string(object_id) + " but its capacity is " + std::to_string(all[0].capacity) + " rows");
+    for (int r = 1; r < world; ++r)
+        if (all[(size_t)r].capacity < all[(size_t)r].rows)
+            return fail(ctx, SPH_E_CAPACITY, "sph_shard_dump: capacity: rank " + std::to_string(r) + " holds " +
+                                             std::to_string(all[(size_t)r].rows) + " rows of object " + std::to_string(object_id) +
+                                             " but its capacity is " + std::to_string(all[(size_t)r].capacity) + " rows");
+    if (mine.rows > 0) {
+        k_dump_scatter<<<n_tiles, DUMP_THREADS, 0, st>>>(ctx->S, own[0], own[1], object_id, counts, x, v);
+        ctx->launches += 1;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    // group 2: every other rank's rows to rank 0, behind the rows of the ranks before it; zero-row transfers skipped
+    bool others = false;
+    for (int r = 1; r < world; ++r) others = others || all[(size_t)r].rows > 0;
+    if (others) {
+        int rc = transport_group(
+            ctx, st, [](int, int) { return SPH_OK; },
+            [&] {
+                if (rank != 0) {
+                    if (mine.rows == 0) return SPH_OK;
+                    const uint64_t bytes = (uint64_t)mine.rows * 12;
+                    if (int rc2 = xfer_send(ctx, st, 0, x, bytes)) return rc2;
+                    return xfer_send(ctx, st, 0, v, bytes);
+                }
+                int64_t row = all[0].rows;
+                for (int r = 1; r < world; ++r) {
+                    const int64_t n = all[(size_t)r].rows;
+                    if (n == 0) continue;
+                    if (int rc2 = xfer_recv(ctx, st, r, x + 3 * row, (uint64_t)n * 12)) return rc2;
+                    if (int rc2 = xfer_recv(ctx, st, r, v + 3 * row, (uint64_t)n * 12)) return rc2;
+                    row += n;
+                }
+                return SPH_OK;
+            });
+        if (rc) return rc;
+    }
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
     return SPH_OK;
 }
 

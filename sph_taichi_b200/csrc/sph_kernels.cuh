@@ -1512,6 +1512,102 @@ __global__ void __launch_bounds__(RIGID_THREADS) k_shard_body_solve(DevParams P,
     }
 }
 
+// =====================================================================================
+// sph_shard_dump: x and v of one object's owned records, compacted in sorted order
+// =====================================================================================
+// Three passes over the owned index range [own0, own1) of the last sort, in tiles of DUMP_TILE consecutive records
+// (one block each, DUMP_ROUNDS rounds of DUMP_THREADS records): count the kept records per tile (ballot + popc), one
+// block scans the tile counts, and the tiles scatter their records to the scanned row offsets.  Within a tile the
+// rows follow the rounds, then the warps, then the lanes, i.e. the index order: the compaction keeps the sorted
+// order and is the same on every run.
+constexpr int DUMP_THREADS = 256;
+constexpr int DUMP_ROUNDS = 4;
+constexpr int DUMP_TILE = DUMP_THREADS * DUMP_ROUNDS;
+constexpr int DUMP_WARPS = DUMP_THREADS / 32;
+
+// a record of the object that this rank owns (the set ShardedSimulation.owned_tensors takes)
+__device__ __forceinline__ bool dump_keep(const DevArrays &S, int i, int32_t object_id) {
+    return __float_as_int(S.x0id[i].w) == object_id && !(__float_as_uint(S.misc[i].z) & FLAG_GHOST);
+}
+
+// counts[b] = kept records of tile b
+__global__ void __launch_bounds__(DUMP_THREADS) k_dump_count(DevArrays S, int own0, int own1, int32_t object_id,
+                                                             int32_t *counts) {
+    __shared__ int warp_rows[DUMP_WARPS];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int base = own0 + blockIdx.x * DUMP_TILE;
+    int rows = 0;  // this warp's kept records (the same in every lane)
+    for (int k = 0; k < DUMP_ROUNDS; ++k) {
+        const int i = base + k * DUMP_THREADS + threadIdx.x;
+        rows += __popc(__ballot_sync(0xffffffffu, i < own1 && dump_keep(S, i, object_id)));
+    }
+    if (lane == 0) warp_rows[w] = rows;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int q = 0; q < DUMP_WARPS; ++q) t += warp_rows[q];
+        counts[blockIdx.x] = t;
+    }
+}
+
+// ONE block: counts[0, n_tiles) -> exclusive prefix sums in place, counts[n_tiles] = the total
+__global__ void __launch_bounds__(DUMP_THREADS) k_dump_scan(int32_t *counts, int n_tiles) {
+    __shared__ int warp_rows[DUMP_WARPS];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int carry = 0;  // rows of the chunks before this one (the same in every thread)
+    for (int c0 = 0; c0 < n_tiles; c0 += DUMP_THREADS) {
+        const int b = c0 + threadIdx.x;
+        const int mine = b < n_tiles ? counts[b] : 0;
+        int incl = mine;
+        for (int d = 1; d < 32; d <<= 1) {
+            const int t = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += t;
+        }
+        if (lane == 31) warp_rows[w] = incl;
+        __syncthreads();
+        int before = carry, chunk = 0;
+        for (int q = 0; q < DUMP_WARPS; ++q) {
+            before += q < w ? warp_rows[q] : 0;
+            chunk += warp_rows[q];
+        }
+        __syncthreads();  // every thread has read warp_rows before the next chunk writes it
+        if (b < n_tiles) counts[b] = before + incl - mine;
+        carry += chunk;
+    }
+    if (threadIdx.x == 0) counts[n_tiles] = carry;
+}
+
+// x[3 r..3 r + 2], v[...] of the kept records, r = the record's row (offsets: k_dump_scan's prefix sums)
+__global__ void __launch_bounds__(DUMP_THREADS) k_dump_scatter(DevArrays S, int own0, int own1, int32_t object_id,
+                                                               const int32_t *offsets, float *x, float *v) {
+    __shared__ int warp_rows[DUMP_ROUNDS][DUMP_WARPS];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int base = own0 + blockIdx.x * DUMP_TILE;
+    unsigned keep[DUMP_ROUNDS];
+#pragma unroll
+    for (int k = 0; k < DUMP_ROUNDS; ++k) {
+        const int i = base + k * DUMP_THREADS + threadIdx.x;
+        keep[k] = __ballot_sync(0xffffffffu, i < own1 && dump_keep(S, i, object_id));
+        if (lane == 0) warp_rows[k][w] = __popc(keep[k]);
+    }
+    __syncthreads();
+    int row = offsets[blockIdx.x];  // first row of this round
+#pragma unroll
+    for (int k = 0; k < DUMP_ROUNDS; ++k) {
+        int r = row + __popc(keep[k] & ((1u << lane) - 1u));
+        for (int q = 0; q < DUMP_WARPS; ++q) {
+            r += q < w ? warp_rows[k][q] : 0;
+            row += warp_rows[k][q];
+        }
+        if ((keep[k] >> lane) & 1u) {
+            const int i = base + k * DUMP_THREADS + threadIdx.x;
+            const float4 a = S.posm[i], b = S.veld[i];
+            x[3 * (size_t)r] = a.x; x[3 * (size_t)r + 1] = a.y; x[3 * (size_t)r + 2] = a.z;
+            v[3 * (size_t)r] = b.x; v[3 * (size_t)r + 1] = b.y; v[3 * (size_t)r + 2] = b.z;
+        }
+    }
+}
+
 // Diagnostics: neighbour-list statistics of the last density pass -> out[4] = {max count, particles in
 // overflow (full-scan fallback), total pairs, particles with a list}.  out must be zeroed by the caller.
 __global__ void k_neighbor_stats(DevParams P, DevArrays S, int32_t *out) {

@@ -34,6 +34,11 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
   eagerly, without overlap; ``SPH_SHARD_GRAPH`` does not apply.  Without the flag, and for DFSPH in any case, dynamic
   solids are refused (``STATIC_SOLIDS_ONLY`` / ``DYNAMIC_SOLIDS_WCSPH_ONLY``): the DFSPH pressure sweeps scatter the
   reactions in every sweep, which would need a reaction exchange per sweep.
+* Output: ``ShardedSimulation.dump(obj_id)`` is ``ParticleSystem.dump`` of a sharded run.  It is collective: every rank
+  compacts x and v of that object's owned records on the device and rank 0 receives them over the engine's own
+  transport (``sph_shard_dump``), in the global cell order of the last sort.  ``run_simulation.py --gpus N`` writes
+  the PLY series and the posed rigid meshes of a sharded run from rank 0 with it; its torch process group (gloo) only
+  carries the NCCL id.  ``gather_owned`` stays the parity tools' gather of whole records.
 
 ``tests/test_slab_gloo.py`` runs the same library code on the CPU: the host-emulated build of the kernels
 (tests/emu/) with ``GlooTransport`` -- torch.distributed point-to-point over gloo -- in place of NCCL.
@@ -311,6 +316,10 @@ class ShardedSimulation:
                      "sph_shard_configure_bodies")
         e._check(e.lib.sph_shard_begin(e.ctx, e._stream()), "sph_shard_begin")
         self.steps_done = 0
+        # the scene's objects and per-object particle counts (build_sharded sets them; dump() sizes rank 0's buffers
+        # from the counts)
+        self.object_collection, self.object_counts = None, None
+        self._dump_bufs = None
 
     def _load(self, arrays, n, uniform_hint):
         """Pack this rank's initial particles (numpy arrays in the reference's field layout)."""
@@ -369,12 +378,17 @@ class ShardedSimulation:
         e._check(e.lib.sph_shard_info(e.ctx, out, C.byref(sent), e._stream()), "sph_shard_info")
         d = {k: int(out[i]) for i, k in enumerate(INFO_KEYS)}
         d["halo_records_sent"] = int(sent.value)
-        st = d["status"]
+        self._raise_on_status(d["status"], d["n_live"])
+        return d
+
+    def _raise_on_status(self, st, n_live):
+        """Raise on the flags of a status word (``info``; ``dump`` passes the OR over all ranks)."""
         if st & STATUS_OUT_OF_GRID:
             raise RuntimeError("a particle left the grid (NaN or outside [0, domain))")
         if st & (STATUS_HALO_CAPACITY | STATUS_SHARD_CAPACITY):
             raise RuntimeError(f"rank {self.rank}: slab capacity exceeded (status {st}: halo_capacity {self.halo_cap}, "
-                               f"capacity {self.n_cap}, live {d['n_live']}); raise capacity_factor")
+                               f"capacity {self.n_cap}{'' if n_live is None else f', live {n_live}'}); "
+                               f"raise capacity_factor")
         if st & STATUS_SHARD_VELOCITY:
             raise RuntimeError(f"rank {self.rank}: a particle moved a whole cell layer in x within one step "
                                f"(|v_x| * dt >= h); the record exchange may have lost it -- reduce timeStepSize")
@@ -383,7 +397,33 @@ class ShardedSimulation:
         if st & STATUS_GHOST_ALIGN:
             raise RuntimeError(f"rank {self.rank}: a neighbour's boundary layers and this rank's ghost layers differ "
                                f"(status {st})")
-        return d
+
+    def dump(self, obj_id):
+        """Collective (call it on every rank between steps with the same ``obj_id``): x and v of object ``obj_id``
+        gathered from every rank over the engine's own transport (``sph_shard_dump``).  Rank 0 returns
+        ``{"position": [n, 3], "velocity": [n, 3]}`` float32 numpy arrays (the keys of ``ParticleSystem.dump``) in the
+        global cell order of the last sort; the other ranks return None.  Every rank sees the OR of all ranks' status
+        words and raises on it as ``info()`` does, so all of them raise together."""
+        e = self.eng
+        if self.rank == 0:
+            if not self.object_counts:
+                raise ValueError("dump() on rank 0 needs object_counts (set by build_sharded) to size its buffers")
+            cap = max(self.object_counts.values())  # rows of the largest object
+        else:
+            cap = self.n_cap  # at most every record this rank holds
+        if self._dump_bufs is None or self._dump_bufs[0].shape[0] != cap:
+            self._dump_bufs = tuple(torch.empty((max(cap, 1), 3), dtype=torch.float32, device=self.device)
+                                    for _ in range(2))
+        x, v = self._dump_bufs
+        rows, status = C.c_int64(0), C.c_uint32(0)
+        rc = e.lib.sph_shard_dump(e.ctx, int(obj_id), C.c_void_p(x.data_ptr()), C.c_void_p(v.data_ptr()), int(cap),
+                                  C.byref(rows), C.byref(status), e._stream())
+        e._check(rc, "sph_shard_dump")
+        self._raise_on_status(int(status.value), None)
+        if self.rank != 0:
+            return None
+        n = int(rows.value)
+        return {"position": x[:n].to("cpu", copy=True).numpy(), "velocity": v[:n].to("cpu", copy=True).numpy()}
 
     @property
     def slab(self):
@@ -445,7 +485,8 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     cfg = SimConfig(scene_dict)
     radius = cfg.get_cfg("particleRadius")
     h = radius * 4.0
-    arrays, _, _, counts = assemble_particles(cfg, 3, 2 * radius)
+    arrays, object_collection, _, counts = assemble_particles(cfg, 3, 2 * radius)
+    object_ids, object_sizes = np.unique(arrays["object_id"], return_counts=True)
     ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
     gx = int(np.ceil(ds / h).astype(int)[0])
     lay = layer_of(arrays["x"], h)
@@ -482,6 +523,8 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     sim = ShardedSimulation(cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, hint, group=group,
                             rebalance_every=rebalance_every, transport=transport, n_fluid=int(fluid.sum()),
                             n_solid=n_solid, bodies=bodies)
+    sim.object_collection = object_collection  # the meshes of the OBJ export (restPosition, restCenterOfMass)
+    sim.object_counts = {int(o): int(k) for o, k in zip(object_ids, object_sizes)}
     return sim, counts["total"]
 
 

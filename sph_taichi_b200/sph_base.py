@@ -12,6 +12,13 @@ import numpy as np
 from .fields import ScalarField
 
 
+def posed_mesh(rest, rest_cm, R, cm):
+    """Vertices of a rigid body's mesh in its current pose (sph_base.py:253-257): cm + R (rest - rest_cm).  The OBJ
+    export of the single engine (``SPHBase._update_mesh``) and of a sharded run (``run_simulation.py --gpus``)."""
+    ret = R @ (rest - rest_cm).T
+    return cm + ret.T
+
+
 class SPHBase:
     def __init__(self, particle_system):
         self.ps = particle_system
@@ -96,8 +103,7 @@ class SPHBase:
             R, cm = ps._engine.rigid_state(ps._body_index[r_obj_id])
         else:
             R, cm = R.cpu().numpy(), self.compute_com_kernel(r_obj_id)
-        ret = R @ (obj["restPosition"] - obj["restCenterOfMass"]).T
-        obj["meshVertices"] = cm + ret.T
+        obj["meshVertices"] = posed_mesh(obj["restPosition"], obj["restCenterOfMass"], R, cm)
 
     # ---- step (sph_base.py:263-271) ----------------------------------------------------------------
     def _fused_step_ok(self):
