@@ -195,6 +195,43 @@ typedef struct SphDfsphStep {
 } SphDfsphStep;
 int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
 
+/* ---- IISPH (implicit incompressible SPH, reference IISPH.py, simulationMethod 3) -------------------------------
+ * The reference's IISPH.py cannot run; these calls implement the formulation DESIGN.md section 10 states (its
+ * deviations from IISPH.py are listed there).  sph_set_iisph(1) puts a context in IISPH mode: the density pass has
+ * DFSPH semantics (no clamp, no EOS), and the WCSPH / DFSPH calls (sph_step, sph_dfsph_*) and every sph_shard_configure*
+ * call refuse the context (IISPH is single-GPU); sph_set_dfsph or sph_set_iisph(0) leave the mode (the context is then
+ * a WCSPH one unless sph_set_dfsph(1) follows; sph_set_iisph(0) on a context that is not in IISPH mode changes
+ * nothing).  The IISPH calls
+ * refuse a context that is not in IISPH mode.  One op per reference method (IISPH.py names):
+ *   0 compute_densities (also builds the neighbour lists)   1 compute_non_pressure_forces (gravity + viscosity)
+ *   2 predict_advection (v* = v + dt a; a_ii, s_i; p = 0.5 p_prev)
+ *   3 pressure_solve_iteration (arg = omega; out_dev = zero-initialised double accumulator of sum |Ap - s| / rho0)
+ *   4 compute_pressure_forces (a^p with the final pressures + reactions on dynamic solids)   5 advect */
+int sph_set_iisph(SphCtx *ctx, int32_t enable);
+int sph_iisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream);
+/* pressure_solve's relaxed Jacobi loop
+ *     it = 0;  while it < max_iterations:  avg = sweep() / n_fluid;  it += 1;  if avg < eta: break
+ * with the loop condition evaluated on the device after every sweep (batches of sweeps as in sph_dfsph_solve; the
+ * first batch is first_batch sweeps).  SYNCHRONOUS: returns it and the last avg (host pointers, may be NULL). */
+int sph_iisph_solve(SphCtx *ctx, int32_t max_iterations, float omega, double eta, int64_t n_fluid, int32_t first_batch,
+                    int32_t *iterations_out, double *avg_err_out, void *stream);
+/* nsteps whole IISPH SPHBase.step()s: neighbour build, moving boundary volumes, ops 0-2, the loop of sph_iisph_solve,
+ * ops 4-5, solve_rigid_body, enforce_boundary_3D(fluid) -- every kernel launched from this one call. */
+typedef struct SphIisphStep {
+    int32_t max_iterations; /* 1000 */
+    float omega;            /* relaxation, 0.5 */
+    double eta;             /* the loop stops when the average error < eta (1e-3) */
+    int64_t n_fluid;        /* fluid particles (the error sum is averaged over them) */
+    int32_t first_batch;    /* in: sweeps launched before the first wait; out: sweeps the last step ran */
+    int32_t iterations;     /* out: sweeps of the last step's loop */
+    double avg_err;         /* out: its last average error */
+} SphIisphStep;
+int sph_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream);
+/* Per-step scratch of the last IISPH kernels, in the current (sorted) order of sph_unpack: a_ii [n], s_i [n] and the
+ * pressure acceleration a^p [n][3] (device pointers, each may be NULL; 0 for solids).  a^p is the last sweep's until
+ * op 4 replaces it with the final one. */
+int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream);
+
 /* ---- x-slab sharding across the GPUs of one node (new; the reference is single-device) -------
  * One process per GPU.  Each rank owns the cell layers [x_lo, x_hi) of the x axis (x-major flattening,
  * particle_system.py:292-294: after the sort every layer is ONE contiguous index range) and keeps

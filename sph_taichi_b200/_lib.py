@@ -27,7 +27,8 @@ ABI_SYMBOLS = [
     "sph_launch_count", "sph_profile_step", "sph_timer_name", "sph_state_offsets", "sph_set_dfsph", "sph_dfsph_op", "sph_dfsph_solve", "sph_dfsph_step",
     "sph_comm_unique_id", "sph_comm_init_nccl", "sph_comm_set_transport", "sph_shard_configure", "sph_shard_begin",
     "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step", "sph_shard_dfsph_step",
-    "sph_shard_transport_stats", "sph_shard_configure_bodies", "sph_shard_dump",
+    "sph_shard_transport_stats", "sph_shard_configure_bodies", "sph_shard_dump", "sph_set_iisph", "sph_iisph_op",
+    "sph_iisph_solve", "sph_iisph_step", "sph_iisph_read",
 ]
 
 
@@ -89,6 +90,11 @@ class SphDfsphStep(C.Structure):
                 ("inv_dt2", C.c_float), ("density0", C.c_float), ("n_fluid", C.c_int64),
                 ("first_batch_v", C.c_int32), ("first_batch", C.c_int32), ("iterations_v", C.c_int32),
                 ("iterations", C.c_int32), ("avg_err_v", C.c_double), ("avg_err", C.c_double)]
+
+
+class SphIisphStep(C.Structure):
+    _fields_ = [("max_iterations", C.c_int32), ("omega", C.c_float), ("eta", C.c_double), ("n_fluid", C.c_int64),
+                ("first_batch", C.c_int32), ("iterations", C.c_int32), ("avg_err", C.c_double)]
 
 
 _lib = None
@@ -162,6 +168,12 @@ def load():
         "sph_shard_dfsph_step": (C.c_int, [vp, i32, C.POINTER(SphDfsphStep), vp]),
         "sph_shard_transport_stats": (C.c_int, [vp, C.POINTER(u64)]),
         "sph_shard_dump": (C.c_int, [vp, i32, vp, vp, i64, C.POINTER(i64), C.POINTER(C.c_uint32), vp]),
+        "sph_set_iisph": (C.c_int, [vp, i32]),
+        "sph_iisph_op": (C.c_int, [vp, i32, C.c_float, vp, vp]),
+        "sph_iisph_solve": (C.c_int, [vp, i32, C.c_float, C.c_double, i64, i32, C.POINTER(i32), C.POINTER(C.c_double),
+                                      vp]),
+        "sph_iisph_step": (C.c_int, [vp, i32, C.POINTER(SphIisphStep), vp]),
+        "sph_iisph_read": (C.c_int, [vp, vp, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

@@ -14,7 +14,7 @@
 #include <string>
 #include <vector>
 
-#include "sph_dfsph.cuh"
+#include "sph_iisph.cuh"
 
 namespace {
 
@@ -30,6 +30,9 @@ const char *const kShardStaticOnly =
 const char *const kShardBodiesWcsph =
     "x-slab sharding of dynamic solids is WCSPH only: the DFSPH pressure sweeps scatter the reactions onto the bodies "
     "in every sweep, which would need a reaction exchange per sweep";
+const char *const kIisphContext =
+    "this context is in IISPH mode (sph_set_iisph): it steps with sph_iisph_op / sph_iisph_solve / sph_iisph_step";
+const char *const kIisphSingleGpu = "IISPH is single-GPU: x-slab sharding supports WCSPH and DFSPH contexts only";
 const char *const kShardBodiesFixed =
     "the body table of a context configured by sph_shard_configure_bodies is fixed: configure a new context";
 
@@ -178,6 +181,7 @@ struct SphCtx {
     cudaStream_t capture_stream = nullptr;  // graphs are captured here (the legacy stream cannot capture)
     bool built = false;  // neighbour structure valid for current positions
     bool list_valid = false;  // neighbour lists valid for current positions (DFSPH kernels)
+    bool iisph = false;  // sph_set_iisph(1): P.dfsph is set too (the density pass of both is the same)
     // x-slab sharding (sph_shard_*)
     SphTransport transport{};
     bool has_transport = false;
@@ -755,6 +759,7 @@ int sph_get_rigid_state(SphCtx *ctx, int32_t body, float *out_dev12, void *strea
 
 int sph_step(SphCtx *ctx, int32_t nsteps, void *stream) {
     if (!ctx || nsteps < 0) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
     if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_step is the fused WCSPH step; DFSPH is driven through sph_dfsph_op");
     if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1057,6 +1062,7 @@ int sph_comm_set_transport(SphCtx *ctx, const SphTransport *t, int32_t rank, int
 int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                         int32_t rebalance_every) {
     if (!ctx) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphSingleGpu);
     if (x_lo < 0 || x_hi > ctx->P.gx || ghost_layers < 1 || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
     // Static solids travel in the records like fluid particles and never change; dynamic solids need moving boundary
@@ -1120,6 +1126,7 @@ extern "C" {
 int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                                int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
     if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphSingleGpu);
     if (x_lo < 0 || x_hi > ctx->P.gx || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
     if (ghost_layers < 3)
@@ -1368,12 +1375,24 @@ int sph_shard_profile_step(SphCtx *ctx, float *ms_out6, void *stream) {
 int sph_set_dfsph(SphCtx *ctx, int32_t enable) {
     if (!ctx) return SPH_E_ARG;
     ctx->P.dfsph = enable ? 1 : 0;
+    ctx->iisph = false;
+    drop_graphs(ctx);
+    return SPH_OK;
+}
+
+int sph_set_iisph(SphCtx *ctx, int32_t enable) {
+    if (!ctx) return SPH_E_ARG;
+    if (enable && ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSingleGpu);
+    if (!enable && !ctx->iisph) return SPH_OK;  // not in IISPH mode: a DFSPH or WCSPH context stays as it is
+    ctx->P.dfsph = enable ? 1 : 0;
+    ctx->iisph = enable != 0;
     drop_graphs(ctx);
     return SPH_OK;
 }
 
 int sph_dfsph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
     if (!ctx) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
     if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called");
     const DevParams &P = ctx->P;
     if (P.n == 0) return SPH_OK;
@@ -1471,44 +1490,93 @@ int shard_dfsph_exchange(SphCtx *c, cudaStream_t st, int what, DfsphCtrl *ctrl, 
     return SPH_OK;
 }
 
-// The Jacobi loop of divergence_solve (mode 0, DFSPH.py:245-254) or pressure_solve (mode 1, DFSPH.py:323-331) with the
-// loop condition on the device: sweeps are launched in batches (the first as long as the caller expects the loop to
-// run -- the previous step's count is a good guess), every sweep ends with k_dfsph_check, sweeps behind the
-// converged one return at once, and the host reads the control block once per batch.
+// A Jacobi loop with its loop condition on the device: sweeps are launched in batches (the first as long as the
+// caller expects the loop to run -- the previous step's count is a good guess), every sweep ends with a check kernel
+// that updates the DfsphCtrl in the workspace scratch block, sweeps behind the converged one return at once, and the
+// host reads the control block once per batch.  sweep(ctrl) launches one sweep, check included, and returns 0 or an
+// SPH_E_* code; each sweep counts `sweep_kernels` kernels (plus whatever it counts itself).
+template <typename Sweep>
+int device_loop(SphCtx *ctx, int32_t first_batch, int sweep_kernels, DfsphCtrl *h, cudaStream_t st, int64_t *kernels,
+                Sweep sweep) {
+    DfsphCtrl *ctrl = reinterpret_cast<DfsphCtrl *>(ctx->ws + ctx->L.off_scratch);
+    *h = DfsphCtrl{};
+    CUDA_TRY(ctx, cudaMemsetAsync(ctrl, 0, sizeof(DfsphCtrl), st));
+    if (ctx->P.n == 0) return SPH_OK;
+    int batch = std::max(1, std::min(first_batch, 64));
+    while (!h->done) {
+        for (int s = 0; s < batch; ++s)
+            if (int rc = sweep(ctrl)) return rc;
+        *kernels += sweep_kernels * (int64_t)batch;
+        CUDA_TRY(ctx, cudaGetLastError());
+        CUDA_TRY(ctx, cudaMemcpyAsync(h, ctrl, sizeof(DfsphCtrl), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(ctx, cudaStreamSynchronize(st));
+        batch = 2;  // the guess was short: continue in pairs
+    }
+    return SPH_OK;
+}
+
+// The Jacobi loop of divergence_solve (mode 0, DFSPH.py:245-254) or pressure_solve (mode 1, DFSPH.py:323-331) as a
+// device_loop whose sweeps end with k_dfsph_check.
 // Sharded (P.slab_on): every sweep also sends the owned boundary layer's velocities after the iteration and its
 // {factor, density_adv} after the density change to the neighbours' first ghost layer, and all-gathers the error
 // partials for k_dfsph_check_ranked; n_fluid is then the global fluid count.
 int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, float offset, int64_t n_fluid,
                      int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
     const DevParams &P = ctx->P;
-    DfsphCtrl *ctrl = reinterpret_cast<DfsphCtrl *>(ctx->ws + ctx->L.off_scratch);
-    *h = DfsphCtrl{};
-    CUDA_TRY(ctx, cudaMemsetAsync(ctrl, 0, sizeof(DfsphCtrl), st));
-    if (P.n == 0) return SPH_OK;
     const int b128 = blocks_for(n_grid, 128);
-    int batch = std::max(1, std::min(first_batch, 64));
-    while (!h->done) {
-        for (int s = 0; s < batch; ++s) {
-            if (mode == 0) k_dfsph_iteration<0><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
-            else k_dfsph_iteration<1><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
-            int rc = shard_dfsph_exchange(ctx, st, DX_VELD, ctrl, false, kernels);
-            if (rc) return rc;
-            if (mode == 0) k_dfsph_density_change_err<0><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
-            else k_dfsph_density_change_err<1><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
-            rc = shard_dfsph_exchange(ctx, st, DX_DFS, ctrl, true, kernels);
-            if (rc) return rc;
-            if (P.slab_on)
-                k_dfsph_check_ranked<<<1, 1, 0, st>>>(ctrl, shard_err_parts(ctx), ctx->rank, ctx->world, (double)n_fluid, eta,
-                                                      max_iterations);
-            else
-                k_dfsph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
-        }
-        *kernels += 3 * (int64_t)batch;
-        CUDA_TRY(ctx, cudaGetLastError());
-        CUDA_TRY(ctx, cudaMemcpyAsync(h, ctrl, sizeof(DfsphCtrl), cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(ctx, cudaStreamSynchronize(st));
-        batch = 2;  // the guess was short: continue in pairs
-    }
+    return device_loop(ctx, first_batch, 3, h, st, kernels, [&](DfsphCtrl *ctrl) {
+        if (mode == 0) k_dfsph_iteration<0><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+        else k_dfsph_iteration<1><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+        int rc = shard_dfsph_exchange(ctx, st, DX_VELD, ctrl, false, kernels);
+        if (rc) return rc;
+        if (mode == 0) k_dfsph_density_change_err<0><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
+        else k_dfsph_density_change_err<1><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
+        rc = shard_dfsph_exchange(ctx, st, DX_DFS, ctrl, true, kernels);
+        if (rc) return rc;
+        if (P.slab_on)
+            k_dfsph_check_ranked<<<1, 1, 0, st>>>(ctrl, shard_err_parts(ctx), ctx->rank, ctx->world, (double)n_fluid, eta,
+                                                  max_iterations);
+        else
+            k_dfsph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
+        return SPH_OK;
+    });
+}
+
+// pressure_solve of IISPH as a device_loop: per sweep k_iisph_pressure_accel<false>, k_iisph_pressure_update (error
+// sum fused) and k_iisph_check.  Single-GPU only.
+int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double eta, int64_t n_fluid, int32_t first_batch,
+                     DfsphCtrl *h, cudaStream_t st, int64_t *kernels) {
+    const DevParams &P = ctx->P;
+    const int b128 = blocks_for(P.n, 128);
+    return device_loop(ctx, first_batch, 3, h, st, kernels, [&](DfsphCtrl *ctrl) {
+        k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+        k_iisph_pressure_update<<<b128, 128, 0, st>>>(P, ctx->S, omega, &ctrl->err, ctrl);
+        k_iisph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
+        return SPH_OK;
+    });
+}
+
+// IISPH.substep (DESIGN section 10): densities (+ lists) -> non-pressure forces without cohesion -> predict_advection
+// -> pressure_solve -> compute_pressure_forces (+ reactions) -> advect.  io: constants in, counts out.
+int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t *kernels) {
+    const DevParams &P = c->P;
+    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
+    launch_pair_density(c, st, kernels);
+    c->list_valid = true;
+    DevParams Pn = P;
+    Pn.sigma = 0.0f;  // IISPH's non-pressure forces are gravity + viscosity: the cohesion term is an exact zero
+    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, c->S);
+    k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, c->S);
+    k_iisph_predict<<<b128, 128, 0, st>>>(P, c->S);
+    *kernels += 3;
+    DfsphCtrl h{};
+    int rc = iisph_solve_loop(c, io->max_iterations, io->omega, io->eta, io->n_fluid, io->first_batch, &h, st, kernels);
+    if (rc) return rc;
+    io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
+    k_iisph_pressure_accel<true><<<b128, 128, 0, st>>>(P, c->S, nullptr);
+    k_iisph_advect<<<b256, 256, 0, st>>>(P, c->S);
+    *kernels += 2;
+    c->built = false; c->list_valid = false;  // positions moved
     return SPH_OK;
 }
 
@@ -1563,6 +1631,24 @@ int launch_dfsph_substep(SphCtx *c, cudaStream_t st, SphDfsphStep *io, int64_t n
     return SPH_OK;
 }
 
+// One single-GPU SPHBase.step() (sph_base.py:263-271) of a solver whose substep launches itself (DFSPH, IISPH):
+//   neighbour build -> moving boundary volumes -> substep() -> solve_rigid_body -> enforce_boundary_3D(fluid)
+template <typename Substep>
+int single_step(SphCtx *ctx, cudaStream_t st, Substep substep) {
+    // ps.initialize_particle_system(), compute_moving_boundary_volume() (sph_base.py:264-265)
+    int rc = launch_neighbor_build(ctx, st, nullptr, &ctx->launches, /*move_acc=*/true);
+    if (rc) return rc;
+    if (ctx->has_dynamic_solids) { rc = launch_boundary_volume(ctx, 1, st, &ctx->launches); if (rc) return rc; }
+    rc = substep();
+    if (rc) return rc;
+    // solve_rigid_body(), enforce_boundary_3D(fluid) (sph_base.py:270-271)
+    if (!ctx->bodies.empty()) { rc = launch_rigid_solve(ctx, st, &ctx->launches); if (rc) return rc; }
+    k_enforce_boundary<<<blocks_for(ctx->P.n, 256), 256, 0, st>>>(ctx->P, ctx->S, /*particle_type=*/1);
+    ctx->launches += 1;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return SPH_OK;
+}
+
 // One sharded DFSPH SPHBase.step() (fluid + static solids; no overlap of the exchanges with computation):
 //   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> substep on owned records + ghosts
 //   -> clamp (owned) -> pack the send ranges -> the record exchange that feeds the next step's classification
@@ -1601,6 +1687,7 @@ extern "C" {
 int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double eta, float offset, int64_t n_fluid,
                     int32_t first_batch, int32_t *iterations_out, int32_t *sweeps_out, double *avg_err_out, void *stream) {
     if (!ctx || (mode != 0 && mode != 1) || n_fluid < 1) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
     if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called");
     if (!ctx->built || !ctx->list_valid)
         return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run sph_neighbor_build and op 0 (compute_densities) first");
@@ -1616,23 +1703,99 @@ int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double et
 
 int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) {
     if (!ctx || !io || nsteps < 0 || io->n_fluid < 1) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
     if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called");
     if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, "this context is sharded: step it with sph_shard_dfsph_step");
     if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int s = 0; s < nsteps; ++s) {
-        // ps.initialize_particle_system(), compute_moving_boundary_volume() (sph_base.py:264-265)
-        int rc = launch_neighbor_build(ctx, st, nullptr, &ctx->launches, /*move_acc=*/true);
+        int rc = single_step(ctx, st, [&] { return launch_dfsph_substep(ctx, st, io, ctx->P.n, &ctx->launches); });
         if (rc) return rc;
-        if (ctx->has_dynamic_solids) { rc = launch_boundary_volume(ctx, 1, st, &ctx->launches); if (rc) return rc; }
-        rc = launch_dfsph_substep(ctx, st, io, ctx->P.n, &ctx->launches);
-        if (rc) return rc;
-        // solve_rigid_body(), enforce_boundary_3D(fluid) (sph_base.py:270-271)
-        if (!ctx->bodies.empty()) { rc = launch_rigid_solve(ctx, st, &ctx->launches); if (rc) return rc; }
-        k_enforce_boundary<<<blocks_for(ctx->P.n, 256), 256, 0, st>>>(ctx->P, ctx->S, /*particle_type=*/1);
-        ctx->launches += 1;
-        CUDA_TRY(ctx, cudaGetLastError());
     }
+    return SPH_OK;
+}
+
+int sph_iisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
+    if (!ctx) return SPH_E_ARG;
+    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    const DevParams &P = ctx->P;
+    if (P.n == 0) return SPH_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
+    if (op < IISPH_COMPUTE_DENSITIES || op > IISPH_ADVECT) return fail(ctx, SPH_E_ARG, "unknown IISPH op");
+    if (!ctx->built) return fail(ctx, SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first");
+    if (op != IISPH_COMPUTE_DENSITIES && op != IISPH_ADVECT && !ctx->list_valid)
+        return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run op 0 (compute_densities) first");
+    if (op == IISPH_PRESSURE_SOLVE_ITERATION && !out_dev) return SPH_E_ARG;
+    DevParams Pn = P;
+    switch (op) {
+        case IISPH_COMPUTE_DENSITIES:
+            launch_pair_density(ctx, st, &ctx->launches);
+            ctx->list_valid = true;
+            break;
+        case IISPH_NON_PRESSURE_FORCES:
+            Pn.sigma = 0.0f;  // gravity + viscosity only
+            k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, ctx->S);
+            ctx->launches += 1;
+            break;
+        case IISPH_PREDICT_ADVECTION:
+            k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, ctx->S);
+            k_iisph_predict<<<b128, 128, 0, st>>>(P, ctx->S);
+            ctx->launches += 2;
+            break;
+        case IISPH_PRESSURE_SOLVE_ITERATION:
+            k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
+            k_iisph_pressure_update<<<b128, 128, 0, st>>>(P, ctx->S, arg, static_cast<double *>(out_dev), nullptr);
+            ctx->launches += 2;
+            break;
+        case IISPH_PRESSURE_FORCES:
+            k_iisph_pressure_accel<true><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
+            ctx->launches += 1;
+            break;
+        case IISPH_ADVECT:
+            k_iisph_advect<<<b256, 256, 0, st>>>(P, ctx->S);
+            ctx->launches += 1;
+            ctx->built = false; ctx->list_valid = false;
+            break;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    return SPH_OK;
+}
+
+int sph_iisph_solve(SphCtx *ctx, int32_t max_iterations, float omega, double eta, int64_t n_fluid, int32_t first_batch,
+                    int32_t *iterations_out, double *avg_err_out, void *stream) {
+    if (!ctx || n_fluid < 1 || max_iterations < 1) return SPH_E_ARG;
+    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    if (!ctx->built || !ctx->list_valid)
+        return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run sph_neighbor_build and op 0 (compute_densities) first");
+    DfsphCtrl h{};
+    int rc = iisph_solve_loop(ctx, max_iterations, omega, eta, n_fluid, first_batch, &h, static_cast<cudaStream_t>(stream),
+                              &ctx->launches);
+    if (rc) return rc;
+    if (iterations_out) *iterations_out = h.iterations;
+    if (avg_err_out) *avg_err_out = h.last_avg;
+    return SPH_OK;
+}
+
+int sph_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream) {
+    if (!ctx || !io || nsteps < 0 || io->n_fluid < 1 || io->max_iterations < 1) return SPH_E_ARG;
+    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    if (ctx->P.n == 0) return SPH_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int s = 0; s < nsteps; ++s) {
+        int rc = single_step(ctx, st, [&] { return launch_iisph_substep(ctx, st, io, &ctx->launches); });
+        if (rc) return rc;
+    }
+    return SPH_OK;
+}
+
+int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) {
+    if (!ctx) return SPH_E_ARG;
+    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    if (ctx->P.n == 0) return SPH_OK;
+    k_iisph_read<<<blocks_for(ctx->P.n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S, a_ii, s, ap);
+    ctx->launches += 1;
+    CUDA_TRY(ctx, cudaGetLastError());
     return SPH_OK;
 }
 

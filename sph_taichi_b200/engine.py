@@ -210,6 +210,31 @@ class Engine:
         """`nsteps` whole DFSPH steps launched from one call; `io` is a _lib.SphDfsphStep (constants in, counts out)."""
         self._check(self.lib.sph_dfsph_step(self.ctx, int(nsteps), C.byref(io), self._stream()), "sph_dfsph_step")
 
+    def set_iisph(self, enable=True):
+        self._check(self.lib.sph_set_iisph(self.ctx, int(bool(enable))), "sph_set_iisph")
+
+    def iisph_op(self, op, arg=0.0, out=None):
+        self._check(self.lib.sph_iisph_op(self.ctx, int(op), float(arg), None if out is None else out.data_ptr(),
+                                          self._stream()), "sph_iisph_op")
+
+    def iisph_solve(self, max_iterations, omega, eta, n_fluid, first_batch):
+        """pressure_solve's Jacobi loop with the loop condition on the device; returns (iterations, last average
+        error).  Synchronous (one wait per batch of sweeps)."""
+        it, avg = C.c_int32(0), C.c_double(0.0)
+        self._check(self.lib.sph_iisph_solve(self.ctx, int(max_iterations), float(omega), float(eta), int(n_fluid),
+                                             int(first_batch), C.byref(it), C.byref(avg), self._stream()),
+                    "sph_iisph_solve")
+        return int(it.value), float(avg.value)
+
+    def iisph_step(self, nsteps, io):
+        """`nsteps` whole IISPH steps launched from one call; `io` is a _lib.SphIisphStep (constants in, counts out)."""
+        self._check(self.lib.sph_iisph_step(self.ctx, int(nsteps), C.byref(io), self._stream()), "sph_iisph_step")
+
+    def iisph_read(self, a_ii=None, s=None, ap=None):
+        """a_ii [n], s [n], a^p [n, 3] (float32 tensors on the engine's device, each may be None), sorted order."""
+        ptr = [None if t is None else t.data_ptr() for t in (a_ii, s, ap)]
+        self._check(self.lib.sph_iisph_read(self.ctx, *ptr, self._stream()), "sph_iisph_read")
+
     def step(self, nsteps=1):
         self._check(self.lib.sph_step(self.ctx, int(nsteps), self._stream()), "sph_step")
 

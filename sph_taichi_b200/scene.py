@@ -155,6 +155,17 @@ def _as_dfsph(sc, dt=0.004):
     return sc
 
 
+def _as_iisph(sc, dt=0.001):
+    sc["Configuration"]["simulationMethod"] = 3
+    sc["Configuration"]["timeStepSize"] = dt
+    return sc
+
+
+def dragon_bath_iisph():
+    """dragon_bath's geometry with the IISPH solver (simulationMethod 3), dt = 1e-3 (DESIGN.md section 10)."""
+    return _as_iisph(dragon_bath())
+
+
 def dragon_bath_dfsph():
     """The reference's dragon_bath_dfsph.json: same geometry, DFSPH, dt = 4e-3."""
     return _as_dfsph(dragon_bath())
@@ -186,6 +197,7 @@ NAMED_SCENES = {
     "armadillo_bath_dynamic": armadillo_bath_dynamic,
     "high_fluid_wcsph": high_fluid_wcsph,
     "dragon_bath_dfsph": dragon_bath_dfsph,
+    "dragon_bath_iisph": dragon_bath_iisph,
     "dragon_bath_dynamic_dfsph": dragon_bath_dynamic_dfsph,
     "high_fluid_dfsph": high_fluid_dfsph,
     "armadillo_bath_dynamic_dfsph": armadillo_bath_dynamic_dfsph,

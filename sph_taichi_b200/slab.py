@@ -69,6 +69,7 @@ STATUS_SOLID_SLOT = 64  # sharded with dynamic solids: two live records with one
 FLAG_FLUID, FLAG_DYNAMIC, FLAG_GHOST = 1, 2, 4  # misc.z bits of a packed record (csrc/sph_common.cuh)
 STATIC_SOLIDS_ONLY = ("x-slab sharding supports static solids only: dynamic solids (shape-matched bodies, advected "
                       "rigid blocks) are single-GPU in WCSPH and DFSPH")
+IISPH_SINGLE_GPU = "IISPH (simulationMethod 3) is single-GPU: x-slab sharding runs WCSPH (0) and DFSPH (4) scenes"
 DYNAMIC_SOLIDS_WCSPH_ONLY = ("x-slab sharding of dynamic solids is WCSPH only: the DFSPH pressure sweeps scatter the "
                              "reactions onto the bodies in every sweep, which would need a reaction exchange per sweep")
 
@@ -483,6 +484,10 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     from .scene import assemble_particles
 
     cfg = SimConfig(scene_dict)
+    method = cfg.get_cfg("simulationMethod")
+    if method not in (0, 4):
+        raise NotImplementedError(IISPH_SINGLE_GPU if method == 3 else
+                                  f"x-slab sharding runs WCSPH (0) and DFSPH (4) scenes, not simulationMethod {method}")
     radius = cfg.get_cfg("particleRadius")
     h = radius * 4.0
     arrays, object_collection, _, counts = assemble_particles(cfg, 3, 2 * radius)
