@@ -175,7 +175,6 @@ struct SphCtx {
     GraphSlot graph[2];
     GraphSlot graph_multi[2];  // GRAPH_UNROLL steps per replay
     int parity = 0;
-    int var_density = 1, var_force = 1;  // 1 = production; 0 = ablation variants (SPH_DENSITY_VARIANT / SPH_FORCE_VARIANT)
     bool time_pair = false;
     cudaEvent_t pair_ev[3] = {nullptr, nullptr, nullptr};
     cudaStream_t capture_stream = nullptr;  // graphs are captured here (the legacy stream cannot capture)
@@ -355,25 +354,23 @@ int launch_neighbor_build(SphCtx *c, cudaStream_t st, StageTimer *tm, int64_t *k
     return SPH_OK;
 }
 
-// density + neighbour lists, then forces (+ integration).  SPH_DENSITY_VARIANT / SPH_FORCE_VARIANT = 0
-// select the ablation variants (second dense loop for the density sum; separate advect kernel).
+// density + neighbour lists, then forces (+ integration).
 // n_grid (sharded DFSPH): the grid covers [0, n_grid) instead of all P.n slots
 void launch_pair_density(SphCtx *c, cudaStream_t st, int64_t *kernels, int split_mode = 0, int64_t n_grid = -1) {
     const DevParams &P = c->P;
     const int blocks = blocks_for(n_grid < 0 ? P.n : n_grid, DENS_WARPS * 32);
-    if (c->var_density == 0) PDL_LAUNCH((k_density_tma<false, false>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
-    else if (P.dfsph || c->var_density == 2) PDL_LAUNCH((k_density_tma<true, false>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
-    else PDL_LAUNCH((k_density_tma<true, true>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
+    if (P.dfsph) PDL_LAUNCH((k_density_tma<false>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
+    else PDL_LAUNCH((k_density_tma<true>), blocks, DENS_WARPS * 32, st, P, c->S, split_mode);
     *kernels += 1;
 }
 void launch_pair_force_and_advect(SphCtx *c, cudaStream_t st, StageTimer *tm, int64_t *kernels, int split_mode = 0) {
     const DevParams &P = c->P;
-    if (P.uniform_fluid && c->var_force != 0) {
+    if (P.uniform_fluid) {
         if (P.slab_on)
-            PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS, true, true>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st, P,
+            PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS, true>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st, P,
                        c->S, split_mode);
         else
-            PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS, true>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st, P, c->S,
+            PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st, P, c->S,
                        split_mode);
         *kernels += 1;
         if (tm) tm->mark(T_ADVECT);
@@ -383,8 +380,7 @@ void launch_pair_force_and_advect(SphCtx *c, cudaStream_t st, StageTimer *tm, in
         }
         return;
     }
-    if (P.uniform_fluid) k_force_packed<FORCE_BATCH, FORCE_THREADS, false><<<blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, 0, st>>>(P, c->S, 0);
-    else k_force_general<4, 128><<<blocks_for(P.n, 128), 128, 0, st>>>(P, c->S);
+    k_force_general<4, 128><<<blocks_for(P.n, 128), 128, 0, st>>>(P, c->S);
     if (tm) tm->mark(T_ADVECT);
     k_advect<true><<<blocks_for(P.n, 256), 256, 0, st>>>(P, c->S);
     *kernels += 2;
@@ -510,17 +506,7 @@ int sph_create(const SphParams *params, int64_t n_max, int64_t n_solid, int32_t 
     c->L = make_layout(n_max, C, n_solid, n_bodies);
     if (c->L.total > workspace_bytes) { delete c; return fail(nullptr, SPH_E_CAPACITY, "workspace too small"); }
     c->ws = static_cast<char *>(workspace);
-    if (const char *v = std::getenv("SPH_DENSITY_VARIANT")) c->var_density = std::atoi(v);
-    if (const char *v = std::getenv("SPH_FORCE_VARIANT")) c->var_force = std::atoi(v);
     c->P = DevParams{};
-    if (const char *v = std::getenv("SPH_COLUMN_ORDER")) {  // experiments: a permutation of 012345678
-        unsigned long long o = 0ull;
-        unsigned seen = 0u;
-        int k = 0;
-        for (; v[k] >= '0' && v[k] <= '8' && k < 9; ++k) { o |= (unsigned long long)(v[k] - '0') << (4 * k); seen |= 1u << (v[k] - '0'); }
-        if (k == 9 && seen == 0x1ffu && v[9] == 0) c->P.col_order = o;
-        else { delete c; return fail(nullptr, SPH_E_ARG, "SPH_COLUMN_ORDER must be a permutation of 012345678"); }
-    }
     derive_params(c);
     c->P.n = 0;
     c->P.n_solid = 0;
@@ -652,7 +638,7 @@ int sph_boundary_volume(SphCtx *ctx, int32_t moving, void *stream) {
 
 int sph_compute_densities(SphCtx *ctx, void *stream) {
     REQUIRE_BUILT(ctx);
-    k_density_simple<false><<<blocks_for(ctx->P.n, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S);
+    k_density_simple<<<blocks_for(ctx->P.n, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S);
     ctx->launches += 1;
     CUDA_TRY(ctx, cudaGetLastError());
     return SPH_OK;
@@ -969,7 +955,7 @@ int shard_bodies_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernel
         }
     }
     launch_pair_density(c, st, kernels, /*split_mode=*/0);
-    PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS, true, true>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st,
+    PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS, true>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st,
                P, c->S, 0);
     *kernels += 1;
     CUDA_TRY(c, cudaGetLastError());

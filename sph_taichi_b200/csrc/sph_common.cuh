@@ -294,6 +294,6 @@ inline void derive_dev_params(DevParams &P, const SphParams &h) {
     }
     P.k1_grad = P.k_dw * P.inv_h; P.wd_norm = P.w_diam / P.k2_w;
     P.opaque_zero = 0;
-    if (P.col_order == 0ull) P.col_order = 0x862075314ull;  // centre, edges, corners (4 1 3 5 7 0 2 6 8)
+    P.col_order = 0x862075314ull;  // centre, edges, corners (4 1 3 5 7 0 2 6 8)
     P.pad = h.h; P.hi_x = h.clamp_hi[0]; P.hi_y = h.clamp_hi[1]; P.hi_z = h.clamp_hi[2];
 }

@@ -423,10 +423,7 @@ __global__ void __launch_bounds__(128) k_boundary_volume(DevParams P, DevArrays 
     if (lane == 0) reinterpret_cast<float *>(S.posm + i)[3] = 1.0f / (P.w0 + part) * 3.0f;
 }
 
-// Densities (WCSPH.py:33-43).  FUSE_EOS additionally applies the clamp + Tait EOS of
-// WCSPH.py:73-76 and initialises the accelerations of non-fluid particles (WCSPH.py:130-137),
-// so the fused force pass can follow immediately.
-template <bool FUSE_EOS>
+// Densities (WCSPH.py:33-43).
 __global__ void __launch_bounds__(128) k_density_simple(DevParams P, DevArrays S) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.n) return;
@@ -436,7 +433,6 @@ __global__ void __launch_bounds__(128) k_density_simple(DevParams P, DevArrays S
     if (!(fl & FLAG_FLUID)) {
         bool dyn = (fl & FLAG_DYNAMIC) != 0;
         S.aux[i] = make_float4(S.veld[i].w, 0.0f, dyn ? -2.0f : -1.0f, 0.0f);
-        if (FUSE_EOS) S.acc[i] = dyn ? make_float4(P.gx_, P.gy_, P.gz_, 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
         return;
     }
     float den = 0.0f;
@@ -448,16 +444,8 @@ __global__ void __launch_bounds__(128) k_density_simple(DevParams P, DevArrays S
     rho += den;
     rho *= P.rho0;
     float vol = mi.x / rho;  // m_j / rho_j with the UNCLAMPED density (viscosity, SURVEY Q4)
-    if (FUSE_EOS) {
-        float rc = fmaxf(rho, P.rho0);
-        float p = tait_pressure(P, rc);
-        reinterpret_cast<float *>(S.veld + i)[3] = rc;
-        reinterpret_cast<float *>(S.misc + i)[1] = p;
-        S.aux[i] = make_float4(vol, p / (rc * rc), mi.x, 0.0f);
-    } else {
-        reinterpret_cast<float *>(S.veld + i)[3] = rho;
-        S.aux[i] = make_float4(vol, 0.0f, mi.x, 0.0f);
-    }
+    reinterpret_cast<float *>(S.veld + i)[3] = rho;
+    S.aux[i] = make_float4(vol, 0.0f, mi.x, 0.0f);
 }
 
 // EOS loop of compute_pressure_forces (WCSPH.py:72-76), un-fused variant
@@ -712,38 +700,34 @@ __device__ void polar_rotation_f64(const double A[9], double R[9], bool &ok) {
     }
 }
 
-// mode 0: compute_com -> out[3];  mode 1: store rest cm;  mode 2: solve_constraints.
-// One gather pass accumulates the raw moments  M = sum m,  X = sum m x,  Q = sum m q,  XQ = sum m x (x) q
-// (q = x_0 - rest_cm); then  cm = X / M  and  A = sum m (x - cm) (x) q = XQ - cm (x) Q  (sph_base.py:182-211).
-// n_step_bodies > 0 (fused step, mode 2, one CTA per body = blockIdx.x): the reference solves the bodies one after
-// the other and clamps ALL dynamic solid particles to the walls after each solve (sph_base.py:247-260), i.e. a
-// particle of body b is clamped b times before its body is solved and n - b times after.  The bodies' particle
-// sets are disjoint and a clamp only looks at the particle itself, so the same sequence runs here per body in ONE
-// launch (3 bodies: 6 launches -> 2, bit-identical).
-__global__ void __launch_bounds__(RIGID_THREADS) k_rigid(DevParams P, DevArrays S, RigidBodyDev *bodies, int body,
-                                                          int mode, float *out, int n_step_bodies) {
-    __shared__ float red[32 * 16];
-    __shared__ float s_R[9];
-    if (n_step_bodies > 0) body = blockIdx.x;
-    const int pre_clamps = n_step_bodies > 0 ? body : 0, post_clamps = n_step_bodies > 0 ? n_step_bodies - body : 0;
-    RigidBodyDev *B = bodies + body;
-    const int b0 = B->solid_begin, b1 = B->solid_end;
-    const float r0 = B->rest_cm[0], r1 = B->rest_cm[1], r2 = B->rest_cm[2];
-    float acc[16];
+// The shape-matching solve, shared by k_rigid and the sharded k_shard_body_solve, which must agree bit for bit.
+// b0, b1 (the body's solid ids) and r0..r2 (its rest cm) are read once by the kernel and passed by value: thread 0
+// writes the body table in between, so reading them from it here would cost extra global loads.
+
+// The clamps the earlier bodies' iterations of the fused step apply to particle i before its body is solved; p holds
+// posm[i] and receives the clamped position.
+__device__ __forceinline__ void rigid_pre_clamps(const DevParams &P, const DevArrays &S, int i, int n, float4 &p) {
+    if (n > 0) {
+        float4 v = S.veld[i];
+        for (int r = 0; r < n; ++r) wall_clamp(P, p, v);
+        S.posm[i] = p;
+        S.veld[i] = v;
+    }
+}
+
+// One gather pass accumulates the raw moments  acc = {M = sum m,  X = sum m x,  Q = sum m q,  XQ = sum m x (x) q}
+// (q = x_0 - rest_cm) over the solid ids [b0, b1): thread t takes b0 + t, b0 + t + blockDim.x, ..., then
+// block_reduce's fixed-order tree, so every thread ends with the same totals.  fetch(s, x, x0, mass) gives the
+// operands of solid id s (x and x_0 in .xyz) or returns false to skip it.
+template <class Fetch>
+__device__ __forceinline__ void rigid_moments(int b0, int b1, float r0, float r1, float r2, float (&acc)[16], float *red,
+                                              Fetch fetch) {
 #pragma unroll
     for (int k = 0; k < 16; ++k) acc[k] = 0.f;
     for (int s = b0 + threadIdx.x; s < b1; s += blockDim.x) {
-        int i = S.solid_slot[s];
-        uint32_t fl = __float_as_uint(S.misc[i].z);
-        if (!(fl & FLAG_DYNAMIC)) continue;  // compute_com counts dynamic rigid particles only (Q8)
-        float4 p = S.posm[i], x0 = S.x0id[i];
-        if (pre_clamps > 0) {  // the clamps the earlier bodies' iterations applied to this particle
-            float4 v = S.veld[i];
-            for (int r = 0; r < pre_clamps; ++r) wall_clamp(P, p, v);
-            S.posm[i] = p;
-            S.veld[i] = v;
-        }
-        float mass = P.m_V0 * S.veld[i].w;
+        float4 p, x0;
+        float mass;
+        if (!fetch(s, p, x0, mass)) continue;
         float q[3] = {x0.x - r0, x0.y - r1, x0.z - r2};
         float x[3] = {p.x, p.y, p.z};
         acc[0] += mass;
@@ -756,15 +740,17 @@ __global__ void __launch_bounds__(RIGID_THREADS) k_rigid(DevParams P, DevArrays 
         }
     }
     block_reduce<16>(acc, red);
+}
+
+// cm = X / M and  A = sum m (x - cm) (x) q = XQ - cm (x) Q  (sph_base.py:182-211).  Thread 0 takes R from the polar
+// decomposition of A (the identity when every entry is below 1e-6) and writes R and cm to B, and R to out when given.
+// Then every thread moves the dynamic particles of [b0, b1) whose slot `owned` accepts to cm + R q and applies
+// post_clamps wall clamps: this body's own and those of the later bodies' iterations in the fused step.
+template <class Owned>
+__device__ __forceinline__ void rigid_solve_apply(const DevParams &P, const DevArrays &S, RigidBodyDev *B, int b0,
+                                                  int b1, float r0, float r1, float r2, const float (&acc)[16],
+                                                  int post_clamps, float *out, float *s_R /* [9] */, Owned owned) {
     const float cmx = acc[1] / acc[0], cmy = acc[2] / acc[0], cmz = acc[3] / acc[0];
-    if (mode == 0) {
-        if (threadIdx.x == 0) { out[0] = cmx; out[1] = cmy; out[2] = cmz; }
-        return;
-    }
-    if (mode == 1) {
-        if (threadIdx.x == 0) { B->rest_cm[0] = cmx; B->rest_cm[1] = cmy; B->rest_cm[2] = cmz; }
-        return;
-    }
     if (threadIdx.x == 0) {
         const float cm[3] = {cmx, cmy, cmz};
         double Ad[9], Rd[9];
@@ -782,7 +768,8 @@ __global__ void __launch_bounds__(RIGID_THREADS) k_rigid(DevParams P, DevArrays 
     }
     __syncthreads();
     for (int s = b0 + threadIdx.x; s < b1; s += blockDim.x) {
-        int i = S.solid_slot[s];
+        const int i = S.solid_slot[s];
+        if (!owned(i)) continue;
         uint32_t fl = __float_as_uint(S.misc[i].z);
         if (!(fl & FLAG_DYNAMIC)) continue;
         float4 p = S.posm[i], x0 = S.x0id[i];
@@ -791,13 +778,50 @@ __global__ void __launch_bounds__(RIGID_THREADS) k_rigid(DevParams P, DevArrays 
         float gy = cmy + (s_R[3] * q0 + s_R[4] * q1 + s_R[5] * q2);
         float gz = cmz + (s_R[6] * q0 + s_R[7] * q1 + s_R[8] * q2);
         p.x += (gx - p.x) * 1.0f; p.y += (gy - p.y) * 1.0f; p.z += (gz - p.z) * 1.0f;
-        if (post_clamps > 0) {  // this body's own clamp and those of the later bodies' iterations
+        if (post_clamps > 0) {
             float4 v = S.veld[i];
             for (int r = 0; r < post_clamps; ++r) wall_clamp(P, p, v);
             S.veld[i] = v;
         }
         S.posm[i] = p;
     }
+}
+
+// mode 0: compute_com -> out[3];  mode 1: store rest cm;  mode 2: solve_constraints.
+// n_step_bodies > 0 (fused step, mode 2, one CTA per body = blockIdx.x): the reference solves the bodies one after
+// the other and clamps ALL dynamic solid particles to the walls after each solve (sph_base.py:247-260), i.e. a
+// particle of body b is clamped b times before its body is solved and n - b times after.  The bodies' particle
+// sets are disjoint and a clamp only looks at the particle itself, so the same sequence runs here per body in ONE
+// launch (3 bodies: 6 launches -> 2, bit-identical).
+__global__ void __launch_bounds__(RIGID_THREADS) k_rigid(DevParams P, DevArrays S, RigidBodyDev *bodies, int body,
+                                                          int mode, float *out, int n_step_bodies) {
+    __shared__ float red[32 * 16];
+    __shared__ float s_R[9];
+    if (n_step_bodies > 0) body = blockIdx.x;
+    const int pre_clamps = n_step_bodies > 0 ? body : 0, post_clamps = n_step_bodies > 0 ? n_step_bodies - body : 0;
+    RigidBodyDev *B = bodies + body;
+    const int b0 = B->solid_begin, b1 = B->solid_end;
+    const float r0 = B->rest_cm[0], r1 = B->rest_cm[1], r2 = B->rest_cm[2];
+    float acc[16];
+    rigid_moments(b0, b1, r0, r1, r2, acc, red, [&](int s, float4 &p, float4 &x0, float &mass) {
+        const int i = S.solid_slot[s];
+        uint32_t fl = __float_as_uint(S.misc[i].z);
+        if (!(fl & FLAG_DYNAMIC)) return false;  // compute_com counts dynamic rigid particles only (Q8)
+        p = S.posm[i]; x0 = S.x0id[i];
+        rigid_pre_clamps(P, S, i, pre_clamps, p);
+        mass = P.m_V0 * S.veld[i].w;
+        return true;
+    });
+    const float cmx = acc[1] / acc[0], cmy = acc[2] / acc[0], cmz = acc[3] / acc[0];
+    if (mode == 0) {
+        if (threadIdx.x == 0) { out[0] = cmx; out[1] = cmy; out[2] = cmz; }
+        return;
+    }
+    if (mode == 1) {
+        if (threadIdx.x == 0) { B->rest_cm[0] = cmx; B->rest_cm[1] = cmy; B->rest_cm[2] = cmz; }
+        return;
+    }
+    rigid_solve_apply(P, S, B, b0, b1, r0, r1, r2, acc, post_clamps, out, s_R, [](int) { return true; });
 }
 
 // =====================================================================================
@@ -885,17 +909,16 @@ __device__ __forceinline__ uint32_t scan_chunk(const DevParams &P, const float4 
 }
 
 // Densities (WCSPH.py:33-43) + clamp and Tait EOS (WCSPH.py:73-76) + neighbour-list build +
-// initial accelerations of non-fluid particles (WCSPH.py:130-137).
-// INLINE_W: the density contribution of a hit is taken from the staged window while flushing the
-// bitmask; otherwise a second dense loop re-gathers the neighbours from global memory.
+// initial accelerations of non-fluid particles (WCSPH.py:130-137).  The density contribution of a hit
+// is taken from the staged window while flushing the bitmask.
 #ifndef DENS_MIN_BLOCKS
 #define DENS_MIN_BLOCKS 8  // H100 sweep of 7-10 blocks/SM: 8 is fastest on dragon_bath and armadillo (DESIGN.md 3.1)
 #endif
-// FASTW (with INLINE_W): the branch-free spline_w_norm() with the 2k factor applied once per particle;
+// FASTW: the branch-free spline_w_norm() with the 2k factor applied once per particle;
 // DFSPH keeps the reference's piecewise form (its solver loops count iterations against the oracle).
 // split_mode (sharded steps): 1 = only the particles within one layer of the send ranges, 2 = only the others,
 // 0 = all that need a density.
-template <bool INLINE_W, bool FASTW>
+template <bool FASTW>
 __global__ void __launch_bounds__(DENS_WARPS * 32, DENS_MIN_BLOCKS) k_density_tma(DevParams P, DevArrays S, int split_mode) {
     pdl_wait();
     __shared__ __align__(128) float4 s_win[DENS_WARPS][2][WIN_CAP + 32];
@@ -987,9 +1010,9 @@ __global__ void __launch_bounds__(DENS_WARPS * 32, DENS_MIN_BLOCKS) k_density_tm
                 S.nbr_list[widx] = jb + b;  // beyond NBR_CAP the last row is overwritten (flagged below)
                 widx = min(widx + (uint32_t)S.npad, widx_cap);
                 ++cnt;
-                if (INLINE_W && FASTW) {
+                if (FASTW) {
                     den = fmaf(pj.w, spline_w_norm(P, r2), den);
-                } else if (INLINE_W) {
+                } else {
                     float r, inv_r;
                     fast_norm(r2, r, inv_r);
                     den += pj.w * w_cubic(P, r);
@@ -1032,38 +1055,11 @@ __global__ void __launch_bounds__(DENS_WARPS * 32, DENS_MIN_BLOCKS) k_density_tm
         // pad the list to a multiple of LIST_PAD with the particle itself: the batched force pass then
         // loads whole batches without per-entry predicates (a self pair contributes exactly zero)
         for (int k = cnt; k % LIST_PAD; ++k) { S.nbr_list[widx] = i; widx += (uint32_t)S.npad; }
-        if (!INLINE_W) {
-            const size_t stride = (size_t)S.npad;
-            const int32_t *lq = S.nbr_list + i;
-            for (int k0 = 0; k0 < cnt; k0 += 4) {
-                float4 pj[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    int j = (k0 + u < cnt) ? lq[(size_t)(k0 + u) * stride] : i;
-                    pj[u] = __ldg(S.posm + j);
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    float rx = pi.x - pj[u].x, ry = pi.y - pj[u].y, rz = pi.z - pj[u].z;
-                    float r2 = rx * rx + ry * ry + rz * rz;
-                    float r, inv_r;
-                    fast_norm(r2, r, inv_r);
-                    float wv = pj[u].w * w_cubic(P, r);
-                    den += (k0 + u < cnt) ? wv : 0.0f;
-                }
-            }
-        }
     } else {
         S.nbr_cnt[i] = NBR_OVERFLOW;
-        if (!INLINE_W) {
-            for_all_neighbors(P, S.posm, S.cell_end, i, pi.x, pi.y, pi.z,
-                              [&](int j, float rx, float ry, float rz, float r2, const float4 &pj) {
-                                  den += pj.w * w_cubic(P, sqrtf(r2));
-                              });
-        }
     }
     float rho = pi.w * P.w0;
-    rho = (INLINE_W && FASTW) ? fmaf(den, P.k2_w, rho) : rho + den;
+    rho = FASTW ? fmaf(den, P.k2_w, rho) : rho + den;
     rho *= P.rho0;
     float vol = mi.x / rho;  // m_j / rho_j with the UNCLAMPED density (viscosity, SURVEY Q4)
     if (P.dfsph) {  // DFSPH.py:39-47: plain density, no clamp, no EOS
@@ -1174,8 +1170,8 @@ __device__ __forceinline__ void force_pair_packed(const DevParams &P, const DevA
 }
 
 // Fused force pass for uniform fluids: ONE 32-byte record gathered per neighbour (LDG.E.256) from the
-// per-step copy fpv.  Because nothing reads posm / veld of OTHER particles here, FUSE_ADVECT lets the
-// epilogue integrate the particle and clamp it to the walls in place (advect + enforce_boundary_3D
+// per-step copy fpv.  Because nothing reads posm / veld of OTHER particles here, the epilogue
+// integrates the particle and clamps it to the walls in place (advect + enforce_boundary_3D
 // (fluid), WCSPH.py:143-149, sph_base.py:149-179) -- one launch and one pass over the state less.
 #ifndef FORCE_MIN_BLOCKS
 #define FORCE_MIN_BLOCKS 6  // H100 sweep of 6-10 blocks/SM and batch 2 / 4: 6 x batch 4 is fastest (DESIGN.md 3.1)
@@ -1209,7 +1205,7 @@ __device__ __forceinline__ void shard_stage_record(const DevParams &P, const Dev
 
 // SHARD: the sharded steps' instantiation (send-range split, staging of the boundary particles); compile-time so
 // that the single-GPU kernel keeps its register budget.
-template <int B, int THREADS, bool FUSE_ADVECT, bool SHARD = false>
+template <int B, int THREADS, bool SHARD = false>
 __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevParams P, DevArrays S,
                                                                             int split_mode) {
     pdl_wait();
@@ -1219,7 +1215,7 @@ __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevP
     if (!(fl & FLAG_FLUID)) {
         // a solid of a send range is staged too, unchanged: k_shard_apply copies the staging back over EVERY record
         // of the send ranges, and the neighbour's ghost copy comes from it (only the static-solid sequence splits)
-        if (SHARD && FUSE_ADVECT && split_mode == 1) shard_stage_record(P, S, i, S.posm[i], S.veld[i], S.x0id[i], mi);
+        if (SHARD && split_mode == 1) shard_stage_record(P, S, i, S.posm[i], S.veld[i], S.x0id[i], mi);
         return;
     }
     if (fl & FLAG_GHOST) return;
@@ -1272,23 +1268,21 @@ __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevP
     }
     float4 a = make_float4(A.npx + A.prx, A.npy + A.pry, A.npz + A.prz, 0.f);
     S.acc[i] = a;
-    if (FUSE_ADVECT) {
-        float4 p = make_float4(pi.x, pi.y, pi.z, P.fluid_mV);
-        float4 v = make_float4(vi.x, vi.y, vi.z, S.veld[i].w);
-        if (fl & FLAG_DYNAMIC) {
-            v.x += P.dt * a.x; v.y += P.dt * a.y; v.z += P.dt * a.z;
-            p.x += P.dt * v.x; p.y += P.dt * v.y; p.z += P.dt * v.z;
-            wall_clamp(P, p, v);
-        }
-        if (SHARD && split_mode == 1) {
-            // sharded boundary pass: the interior DENSITIES are still to come and read the positions of these
-            // particles, so the advanced state goes to the send staging only (this IS the pack step; the halo
-            // exchange starts right after this kernel) and k_shard_apply copies it back later
-            shard_stage_record(P, S, i, p, v, S.x0id[i], mi);
-        } else if (fl & FLAG_DYNAMIC) {
-            S.posm[i] = p;
-            S.veld[i] = v;
-        }
+    float4 p = make_float4(pi.x, pi.y, pi.z, P.fluid_mV);
+    float4 v = make_float4(vi.x, vi.y, vi.z, S.veld[i].w);
+    if (fl & FLAG_DYNAMIC) {
+        v.x += P.dt * a.x; v.y += P.dt * a.y; v.z += P.dt * a.z;
+        p.x += P.dt * v.x; p.y += P.dt * v.y; p.z += P.dt * v.z;
+        wall_clamp(P, p, v);
+    }
+    if (SHARD && split_mode == 1) {
+        // sharded boundary pass: the interior DENSITIES are still to come and read the positions of these
+        // particles, so the advanced state goes to the send staging only (this IS the pack step; the halo
+        // exchange starts right after this kernel) and k_shard_apply copies it back later
+        shard_stage_record(P, S, i, p, v, S.x0id[i], mi);
+    } else if (fl & FLAG_DYNAMIC) {
+        S.posm[i] = p;
+        S.veld[i] = v;
     }
     };  // one particle
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1302,7 +1296,7 @@ __global__ void __launch_bounds__(THREADS, FORCE_MIN_BLOCKS) k_force_packed(DevP
     one(i);
 }
 
-// advect (WCSPH.py:143-149) for the dynamic SOLID particles only (companion of FUSE_ADVECT)
+// advect (WCSPH.py:143-149) for the dynamic SOLID particles only (k_force_packed advects the fluid)
 __global__ void k_advect_solids(DevParams P, DevArrays S) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.n_solid) return;
@@ -1401,7 +1395,8 @@ __global__ void __launch_bounds__(128) k_shard_reactions(DevParams P, DevArrays 
 // summed in a fixed order over the solid ids (thread t of a 1024-thread CTA takes s = b0 + t, b0 + t + 1024, ..., then
 // a fixed-order tree), and that rounding moves cm by ~1e-6 of the domain per step even in free fall -- a reduction in
 // any other order or precision drifts from the single engine within a hundred steps and diverges after an impact.
-// So every rank gathers the records of ALL body particles and repeats k_rigid's reduction on them.
+// So every rank gathers the records of ALL body particles and runs k_rigid's rigid_moments and rigid_solve_apply on
+// them.
 
 // Offset of body b's particles in the gathered table (the bodies' particles in body order, then solid-id order).
 __device__ __forceinline__ int shard_body_offset(const RigidBodyDev *bodies, int b) {
@@ -1426,12 +1421,7 @@ __global__ void k_shard_body_pack(DevParams P, DevArrays S, const RigidBodyDev *
             continue;
         }
         float4 p = S.posm[i];
-        if (pre_clamps > 0) {
-            float4 v = S.veld[i];
-            for (int k = 0; k < pre_clamps; ++k) wall_clamp(P, p, v);
-            S.posm[i] = p;
-            S.veld[i] = v;
-        }
+        rigid_pre_clamps(P, S, i, pre_clamps, p);
         const float4 x0 = S.x0id[i];
         r[0] = make_float4(p.x, p.y, p.z, P.m_V0 * S.veld[i].w);
         r[1] = make_float4(x0.x, x0.y, x0.z, 1.0f);
@@ -1452,64 +1442,20 @@ __global__ void __launch_bounds__(RIGID_THREADS) k_shard_body_solve(DevParams P,
     const int b0 = B->solid_begin, b1 = B->solid_end, off = shard_body_offset(bodies, body);
     const float r0 = B->rest_cm[0], r1 = B->rest_cm[1], r2 = B->rest_cm[2];
     float acc[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) acc[k] = 0.f;
-    for (int s = b0 + threadIdx.x; s < b1; s += blockDim.x) {
+    // captures by value: by reference, the table search re-reads `tables` from the parameter space every iteration
+    rigid_moments(b0, b1, r0, r1, r2, acc, red, [=](int s, float4 &p, float4 &x0, float &mass) {
         const float4 *rec = nullptr;
         for (int r = 0; r < world && !rec; ++r) {
             const float4 *t = tables + 2 * ((size_t)r * n_rec + off + (s - b0));
             if (t[1].w != 0.0f) rec = t;
         }
-        if (!rec) continue;  // not a dynamic particle (k_rigid skips it too)
-        const float4 p = rec[0], x0 = rec[1];
-        float mass = p.w;
-        float q[3] = {x0.x - r0, x0.y - r1, x0.z - r2};
-        float x[3] = {p.x, p.y, p.z};
-        acc[0] += mass;
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-            acc[1 + r] += mass * x[r];
-            acc[4 + r] += mass * q[r];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) acc[7 + 3 * r + c] += mass * x[r] * q[c];
-        }
-    }
-    block_reduce<16>(acc, red);
-    const float cmx = acc[1] / acc[0], cmy = acc[2] / acc[0], cmz = acc[3] / acc[0];
-    if (threadIdx.x == 0) {
-        const float cm[3] = {cmx, cmy, cmz};
-        double Ad[9], Rd[9];
-        for (int r = 0; r < 3; ++r)
-            for (int c = 0; c < 3; ++c) Ad[3 * r + c] = (double)acc[7 + 3 * r + c] - (double)cm[r] * (double)acc[4 + c];
-        bool ok;
-        polar_rotation_f64(Ad, Rd, ok);
-        if (!ok) atomicOr(S.status, SPH_STATUS_BAD_POLAR);
-        bool all_small = true;
-        float Rf[9];
-        for (int k = 0; k < 9; ++k) { Rf[k] = (float)Rd[k]; if (!(fabsf(Rf[k]) < 1e-6f)) all_small = false; }
-        if (all_small) { for (int k = 0; k < 9; ++k) Rf[k] = (k % 4 == 0) ? 1.0f : 0.0f; }
-        for (int k = 0; k < 9; ++k) { s_R[k] = Rf[k]; B->R[k] = Rf[k]; }
-        B->cm[0] = cmx; B->cm[1] = cmy; B->cm[2] = cmz;
-    }
-    __syncthreads();
-    for (int s = b0 + threadIdx.x; s < b1; s += blockDim.x) {
-        const int i = S.solid_slot[s];
-        if (!shard_owned_index(S, i)) continue;
-        uint32_t fl = __float_as_uint(S.misc[i].z);
-        if (!(fl & FLAG_DYNAMIC)) continue;
-        float4 p = S.posm[i], x0 = S.x0id[i];
-        float q0 = x0.x - r0, q1 = x0.y - r1, q2 = x0.z - r2;
-        float gx = cmx + (s_R[0] * q0 + s_R[1] * q1 + s_R[2] * q2);
-        float gy = cmy + (s_R[3] * q0 + s_R[4] * q1 + s_R[5] * q2);
-        float gz = cmz + (s_R[6] * q0 + s_R[7] * q1 + s_R[8] * q2);
-        p.x += (gx - p.x) * 1.0f; p.y += (gy - p.y) * 1.0f; p.z += (gz - p.z) * 1.0f;
-        if (post_clamps > 0) {
-            float4 v = S.veld[i];
-            for (int r = 0; r < post_clamps; ++r) wall_clamp(P, p, v);
-            S.veld[i] = v;
-        }
-        S.posm[i] = p;
-    }
+        if (!rec) return false;  // not a dynamic particle (k_rigid skips it too)
+        p = rec[0]; x0 = rec[1];
+        mass = p.w;
+        return true;
+    });
+    rigid_solve_apply(P, S, B, b0, b1, r0, r1, r2, acc, post_clamps, nullptr, s_R,
+                      [&](int i) { return shard_owned_index(S, i); });
 }
 
 // =====================================================================================
