@@ -198,11 +198,14 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
 /* ---- IISPH (implicit incompressible SPH, reference IISPH.py, simulationMethod 3) -------------------------------
  * The reference's IISPH.py cannot run; these calls implement the formulation DESIGN.md section 10 states (its
  * deviations from IISPH.py are listed there).  sph_set_iisph(1) puts a context in IISPH mode: the density pass has
- * DFSPH semantics (no clamp, no EOS), and the WCSPH / DFSPH calls (sph_step, sph_dfsph_*) and every sph_shard_configure*
- * call refuse the context (IISPH is single-GPU); sph_set_dfsph or sph_set_iisph(0) leave the mode (the context is then
- * a WCSPH one unless sph_set_dfsph(1) follows; sph_set_iisph(0) on a context that is not in IISPH mode changes
- * nothing).  The IISPH calls
- * refuse a context that is not in IISPH mode.  One op per reference method (IISPH.py names):
+ * DFSPH semantics (no clamp, no EOS), and the WCSPH / DFSPH calls (sph_step, sph_dfsph_*, sph_shard_step,
+ * sph_shard_profile_step, sph_shard_dfsph_step) and sph_shard_configure_bodies refuse the context (dynamic solids in
+ * IISPH are single-GPU); sph_set_dfsph or sph_set_iisph(0) leave the mode (the context is then a WCSPH one unless
+ * sph_set_dfsph(1) follows; sph_set_iisph(0) on a context that is not in IISPH mode changes nothing).  An IISPH context
+ * may be x-slab sharded: sph_set_iisph(1) BEFORE sph_shard_configure (it is refused on a sharded context), then
+ * sph_shard_iisph_step (below).  The IISPH calls refuse a context that is not in IISPH mode, and sph_iisph_op,
+ * sph_iisph_solve and sph_iisph_step refuse a sharded one (their grids cover the capacity, ghosts and trash included).
+ * One op per reference method (IISPH.py names):
  *   0 compute_densities (also builds the neighbour lists)   1 compute_non_pressure_forces (gravity + viscosity)
  *   2 predict_advection (v* = v + dt a; a_ii, s_i; p = 0.5 p_prev)
  *   3 pressure_solve_iteration (arg = omega; out_dev = zero-initialised double accumulator of sum |Ap - s| / rho0)
@@ -264,6 +267,10 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream);
  * -- two per Jacobi sweep.  The loops' error sums are all-gathered and added in rank order, so every rank takes the
  * same convergence decision and issues the same transport calls.
  *
+ * IISPH contexts (sph_set_iisph(1) before sph_shard_configure; fluid + static solids) step with sph_shard_iisph_step:
+ * the same step shape as sph_shard_dfsph_step, with the outermost owned layer's v* sent after predict_velocity, its
+ * aux word (p / rho^2) after the diagonal / source pass and after every pressure update, and its acc word (a^p) after
+ * every pressure-acceleration pass -- two exchanges per relaxed Jacobi sweep.
  *
  * The exchange goes through an SphTransport: NCCL point-to-point (libnccl.so.2 is dlopen'ed; the communicator
  * belongs to this library, created from an id the caller distributes), or caller-supplied functions (the CPU
@@ -312,6 +319,18 @@ int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream);
  * moves a whole cell layer in x in one step sets SPH_STATUS_SHARD_VELOCITY (the record exchange would lose it);
  * sph_shard_info reports the status word. */
 int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
+/* nsteps sharded IISPH SPHBase.step()s of an IISPH context (fluid + static solids): the step of sph_iisph_step with
+ * `io` used the same way, except that io->n_fluid is the GLOBAL fluid count (all ranks).  One step:
+ *     plan -> classify + sort -> info -> DX ranges -> ghost alignment -> densities (owned + first ghost layer)
+ *     -> non-pressure forces -> predict velocity -> [v*] -> diagonal, source, warm start -> [aux]
+ *     -> loop { pressure acceleration -> [acc] -> pressure update (error partial) -> [aux + all-gather of the
+ *               partials] -> the loop check on the partials added in rank order }
+ *     -> final pressure acceleration -> advect -> fluid wall clamp -> the record exchange
+ * ([w] = the 16-byte words w of the outermost owned layer sent to the neighbours' first ghost layer.)  Every rank
+ * returns the same iterations, first_batch and avg_err values.  Eager launches with one host wait per batch of sweeps
+ * (SPH_SHARD_GRAPH does not apply).  A particle that moves a whole cell layer in x in one step sets
+ * SPH_STATUS_SHARD_VELOCITY.  The warm-start pressure travels in the records (misc.y), so migrating particles keep it. */
+int sph_shard_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream);
 /* out2 = {transport groups this context issued from the host, bytes it sent in them}; graph replays of
  * sph_shard_step (SPH_SHARD_GRAPH=1) re-issue the captured groups without counting them */
 int sph_shard_transport_stats(SphCtx *ctx, uint64_t *out2);
@@ -338,7 +357,7 @@ int sph_shard_info(SphCtx *ctx, int32_t *out16, uint64_t *out_sent, void *stream
  * rank's status word (sph_shard_info's), the same on every rank, also when SPH_E_CAPACITY is returned.
  * sph_shard_transport_stats counts the bytes like any other group: this rank sends (world - 1) * 16 bytes of headers,
  * plus, on ranks other than rank 0, 24 bytes (x and v, 3 float32 each) per row it holds.  Launches nothing into
- * sph_shard_step's graphs; works on WCSPH, DFSPH and sph_shard_configure_bodies contexts.  Single-GPU contexts are
+ * sph_shard_step's graphs; works on WCSPH, DFSPH, IISPH and sph_shard_configure_bodies contexts.  Single-GPU contexts are
  * refused (they have sph_unpack_xv); capacity < 0 or a null pointer returns SPH_E_ARG. */
 int sph_shard_dump(SphCtx *ctx, int32_t object_id, float *x, float *v, int64_t capacity, int64_t *rows_out,
                    uint32_t *status_out, void *stream);

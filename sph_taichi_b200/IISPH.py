@@ -29,6 +29,16 @@ MAX_ERROR = 1e-3
 FIRST_BATCH = 4  # first batch of sweeps before a step has counted them
 
 
+def iisph_step_io(n_fluid, first_batch=FIRST_BATCH, *, omega=OMEGA, max_iterations=MAX_ITERATIONS,
+                  max_error=MAX_ERROR):
+    """The ``SphIisphStep`` of ``sph_iisph_step`` / ``sph_shard_iisph_step``: the loop's limit, relaxation and threshold
+    (eta = the average error below which pressure_solve stops), the fluid count the error is averaged over (sharded:
+    the fluid particles of ALL ranks) and the first batch of sweeps."""
+    from ._lib import SphIisphStep
+    return SphIisphStep(max_iterations=int(max_iterations), omega=float(omega), eta=float(max_error),
+                        n_fluid=int(n_fluid), first_batch=int(first_batch))
+
+
 class _ScratchField:
     """Read-only per-particle scratch of the last IISPH kernels (a_ii, s_i or a^p), in the public fields' order."""
 
@@ -76,9 +86,8 @@ class IISPHSolver(SPHBase):
 
     def step_io(self):
         """The ``SphIisphStep`` of ``sph_iisph_step`` from this solver's constants."""
-        from ._lib import SphIisphStep
-        return SphIisphStep(max_iterations=int(self.max_iterations), omega=float(self.omega), eta=float(self.max_error),
-                            n_fluid=int(self.ps.fluid_particle_num), first_batch=int(self._sweeps_guess))
+        return iisph_step_io(self.ps.fluid_particle_num, self._sweeps_guess, omega=self.omega,
+                             max_iterations=self.max_iterations, max_error=self.max_error)
 
     # ---- kernels (IISPH.py names) ------------------------------------------------------------
     def compute_densities(self):

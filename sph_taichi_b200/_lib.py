@@ -28,7 +28,7 @@ ABI_SYMBOLS = [
     "sph_comm_unique_id", "sph_comm_init_nccl", "sph_comm_set_transport", "sph_shard_configure", "sph_shard_begin",
     "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step", "sph_shard_dfsph_step",
     "sph_shard_transport_stats", "sph_shard_configure_bodies", "sph_shard_dump", "sph_set_iisph", "sph_iisph_op",
-    "sph_iisph_solve", "sph_iisph_step", "sph_iisph_read",
+    "sph_iisph_solve", "sph_iisph_step", "sph_iisph_read", "sph_shard_iisph_step",
 ]
 
 
@@ -174,6 +174,7 @@ def load():
                                       vp]),
         "sph_iisph_step": (C.c_int, [vp, i32, C.POINTER(SphIisphStep), vp]),
         "sph_iisph_read": (C.c_int, [vp, vp, vp, vp, vp]),
+        "sph_shard_iisph_step": (C.c_int, [vp, i32, C.POINTER(SphIisphStep), vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

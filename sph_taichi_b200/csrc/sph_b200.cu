@@ -32,7 +32,14 @@ const char *const kShardBodiesWcsph =
     "in every sweep, which would need a reaction exchange per sweep";
 const char *const kIisphContext =
     "this context is in IISPH mode (sph_set_iisph): it steps with sph_iisph_op / sph_iisph_solve / sph_iisph_step";
-const char *const kIisphSingleGpu = "IISPH is single-GPU: x-slab sharding supports WCSPH and DFSPH contexts only";
+// sharded IISPH (sph_shard_iisph_step) runs fluid and static solids; the single-GPU IISPH calls launch over the
+// capacity of a sharded context and would step its ghost and trash records too
+const char *const kIisphSharded = "this IISPH context is sharded: step it with sph_shard_iisph_step";
+const char *const kIisphShardStep =
+    "this context is in IISPH mode (sph_set_iisph): a sharded IISPH context steps with sph_shard_iisph_step";
+const char *const kIisphAfterConfigure = "call sph_set_iisph(1) before sph_shard_configure, not on a sharded context";
+const char *const kShardBodiesIisph =
+    "x-slab sharding of dynamic solids is WCSPH only: dynamic solids in IISPH are single-GPU";
 const char *const kShardBodiesFixed =
     "the body table of a context configured by sph_shard_configure_bodies is fixed: configure a new context";
 
@@ -1048,7 +1055,6 @@ int sph_comm_set_transport(SphCtx *ctx, const SphTransport *t, int32_t rank, int
 int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                         int32_t rebalance_every) {
     if (!ctx) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphSingleGpu);
     if (x_lo < 0 || x_hi > ctx->P.gx || ghost_layers < 1 || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
     // Static solids travel in the records like fluid particles and never change; dynamic solids need moving boundary
@@ -1112,7 +1118,7 @@ extern "C" {
 int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                                int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
     if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphSingleGpu);
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kShardBodiesIisph);
     if (x_lo < 0 || x_hi > ctx->P.gx || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
     if (ghost_layers < 3)
@@ -1176,6 +1182,7 @@ int sph_halo_exchange(SphCtx *ctx, void *stream) {
 int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream) {
     REQUIRE_SHARD(ctx);
     if (nsteps < 0) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphShardStep);
     if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_step is the WCSPH step; DFSPH contexts step with sph_shard_dfsph_step");
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1335,6 +1342,7 @@ int sph_shard_dump(SphCtx *ctx, int32_t object_id, float *x, float *v, int64_t c
 int sph_shard_profile_step(SphCtx *ctx, float *ms_out6, void *stream) {
     REQUIRE_SHARD(ctx);
     if (!ms_out6) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphShardStep);
     if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_profile_step times the WCSPH step");
     if (ctx->shard_bodies)
         return fail(ctx, SPH_E_ARG, "sph_shard_profile_step times the static-solid WCSPH step, not the step of a context "
@@ -1368,7 +1376,7 @@ int sph_set_dfsph(SphCtx *ctx, int32_t enable) {
 
 int sph_set_iisph(SphCtx *ctx, int32_t enable) {
     if (!ctx) return SPH_E_ARG;
-    if (enable && ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSingleGpu);
+    if (enable && ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphAfterConfigure);
     if (!enable && !ctx->iisph) return SPH_OK;  // not in IISPH mode: a DFSPH or WCSPH context stays as it is
     ctx->P.dfsph = enable ? 1 : 0;
     ctx->iisph = enable != 0;
@@ -1429,8 +1437,8 @@ inline double *shard_err_parts(const SphCtx *c) { return reinterpret_cast<double
 // One exchange of the sharded DFSPH step with both neighbours: pack -> one transport group -> unpack.
 //   DX_ALIGN: the ghost alignment (4 record arrays of the sgw boundary layers + a 16-byte header per side), received
 //             into the receive regions behind the live records, which stay unused until the end-of-step exchange;
-//   DX_VELD / DX_DFS: one 16-byte word per particle of the outermost owned layer, received into the second staging
-//             array.
+//   DX_VELD / DX_DFS / DX_ACC / DX_AUX: one 16-byte word per particle of the outermost owned layer, received into the
+//             second staging array.
 // Fixed-size messages (align_cap / sweep_cap records), so both sides always agree on the byte counts.  gather_err: the
 // same group also sends this rank's fp64 error partial (ctrl->err) to every other rank and receives theirs into
 // shard_err_parts() -- an all-gather of 8 bytes with plain send / recv.  ctrl (may be NULL): the pack and unpack of a
@@ -1528,35 +1536,55 @@ int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, 
     });
 }
 
-// pressure_solve of IISPH as a device_loop: per sweep k_iisph_pressure_accel<false>, k_iisph_pressure_update (error
-// sum fused) and k_iisph_check.  Single-GPU only.
+// pressure_solve of IISPH over the sorted records [0, n_grid) as a device_loop: per sweep k_iisph_pressure_accel<false>,
+// k_iisph_pressure_update (error sum fused) and k_iisph_check.
+// Sharded (P.slab_on): every sweep also sends the outermost owned layer's acc = {a^p, 1} after the first pass and its
+// aux = {.., p / rho^2, ..} after the second to the neighbours' first ghost layer, and all-gathers the error partials
+// for k_iisph_check_ranked; n_fluid is then the global fluid count.
 int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double eta, int64_t n_fluid, int32_t first_batch,
-                     DfsphCtrl *h, cudaStream_t st, int64_t *kernels) {
+                     DfsphCtrl *h, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
     const DevParams &P = ctx->P;
-    const int b128 = blocks_for(P.n, 128);
+    const int b128 = blocks_for(n_grid, 128);
     return device_loop(ctx, first_batch, 3, h, st, kernels, [&](DfsphCtrl *ctrl) {
         k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+        int rc = shard_dfsph_exchange(ctx, st, DX_ACC, ctrl, false, kernels);
+        if (rc) return rc;
         k_iisph_pressure_update<<<b128, 128, 0, st>>>(P, ctx->S, omega, &ctrl->err, ctrl);
-        k_iisph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
+        rc = shard_dfsph_exchange(ctx, st, DX_AUX, ctrl, true, kernels);
+        if (rc) return rc;
+        if (P.slab_on)
+            k_iisph_check_ranked<<<1, 1, 0, st>>>(ctrl, shard_err_parts(ctx), ctx->rank, ctx->world, (double)n_fluid, eta,
+                                                  max_iterations);
+        else
+            k_iisph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
         return SPH_OK;
     });
 }
 
-// IISPH.substep (DESIGN section 10): densities (+ lists) -> non-pressure forces without cohesion -> predict_advection
-// -> pressure_solve -> compute_pressure_forces (+ reactions) -> advect.  io: constants in, counts out.
-int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t *kernels) {
+// IISPH.substep (DESIGN section 10) over the sorted records [0, n_grid): densities (+ lists) -> non-pressure forces
+// without cohesion -> predict_advection -> pressure_solve -> compute_pressure_forces (+ reactions) -> advect.  io:
+// constants in, counts out.  The exchanges run only on a sharded context: v* after predict_velocity (read by
+// k_iisph_predict), aux after k_iisph_predict (the warm-start p / rho^2 the first sweep reads), then the two of every
+// sweep.  compute_pressure_forces reads the aux words the converged sweep sent; nothing reads a ghost value after it.
+int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n_grid, int64_t *kernels) {
     const DevParams &P = c->P;
-    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
-    launch_pair_density(c, st, kernels);
+    const int b128 = blocks_for(n_grid, 128), b256 = blocks_for(n_grid, 256);
+    launch_pair_density(c, st, kernels, /*split_mode=*/0, n_grid);
     c->list_valid = true;
     DevParams Pn = P;
     Pn.sigma = 0.0f;  // IISPH's non-pressure forces are gravity + viscosity: the cohesion term is an exact zero
     k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, c->S);
     k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, c->S);
+    *kernels += 2;
+    int rc = shard_dfsph_exchange(c, st, DX_VELD, nullptr, false, kernels);
+    if (rc) return rc;
     k_iisph_predict<<<b128, 128, 0, st>>>(P, c->S);
-    *kernels += 3;
+    *kernels += 1;
+    rc = shard_dfsph_exchange(c, st, DX_AUX, nullptr, false, kernels);
+    if (rc) return rc;
     DfsphCtrl h{};
-    int rc = iisph_solve_loop(c, io->max_iterations, io->omega, io->eta, io->n_fluid, io->first_batch, &h, st, kernels);
+    rc = iisph_solve_loop(c, io->max_iterations, io->omega, io->eta, io->n_fluid, io->first_batch, &h, st, n_grid,
+                          kernels);
     if (rc) return rc;
     io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
     k_iisph_pressure_accel<true><<<b128, 128, 0, st>>>(P, c->S, nullptr);
@@ -1635,10 +1663,12 @@ int single_step(SphCtx *ctx, cudaStream_t st, Substep substep) {
     return SPH_OK;
 }
 
-// One sharded DFSPH SPHBase.step() (fluid + static solids; no overlap of the exchanges with computation):
-//   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> substep on owned records + ghosts
+// One sharded SPHBase.step() of a solver whose substep launches itself (DFSPH, IISPH; fluid + static solids; no
+// overlap of the exchanges with computation):
+//   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> substep(n_grid) on owned records + ghosts
 //   -> clamp (owned) -> pack the send ranges -> the record exchange that feeds the next step's classification
-int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, SphDfsphStep *io, bool wide, int64_t *kernels) {
+template <typename Substep>
+int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels, Substep substep) {
     k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
     *kernels += 1;
     int rc = launch_neighbor_build(c, st, nullptr, kernels, /*move_acc=*/false);
@@ -1651,12 +1681,12 @@ int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, SphDfsphStep *io, bool wide
     rc = shard_dfsph_exchange(c, st, DX_ALIGN, nullptr, false, kernels);
     if (rc) return rc;
     // The step waits on the host once per batch of sweeps anyway; one more short wait here for the live count lets
-    // every DFSPH launch cover [0, n_live) -- owned records and ghosts -- instead of the whole capacity.
+    // every substep launch cover [0, n_live) -- owned records and ghosts -- instead of the whole capacity.
     int32_t n_live = 0;
     CUDA_TRY(c, cudaMemcpyAsync(&n_live, c->S.sd + SD_N_LIVE, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(c, cudaStreamSynchronize(st));
     const int64_t n_grid = std::min<int64_t>(std::max<int32_t>(n_live, 1), P.n);
-    rc = launch_dfsph_substep(c, st, io, n_grid, kernels);
+    rc = substep(n_grid);
     if (rc) return rc;
     // enforce_boundary_3D(fluid), sph_base.py:271 (no rigid solve before it: sharded contexts hold static solids only)
     k_enforce_boundary<<<blocks_for(n_grid, 256), 256, 0, st>>>(P, c->S, /*particle_type=*/1);
@@ -1704,6 +1734,7 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) 
 int sph_iisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
     if (!ctx) return SPH_E_ARG;
     if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSharded);
     const DevParams &P = ctx->P;
     if (P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1752,11 +1783,12 @@ int sph_iisph_solve(SphCtx *ctx, int32_t max_iterations, float omega, double eta
                     int32_t *iterations_out, double *avg_err_out, void *stream) {
     if (!ctx || n_fluid < 1 || max_iterations < 1) return SPH_E_ARG;
     if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSharded);
     if (!ctx->built || !ctx->list_valid)
         return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run sph_neighbor_build and op 0 (compute_densities) first");
     DfsphCtrl h{};
     int rc = iisph_solve_loop(ctx, max_iterations, omega, eta, n_fluid, first_batch, &h, static_cast<cudaStream_t>(stream),
-                              &ctx->launches);
+                              ctx->P.n, &ctx->launches);
     if (rc) return rc;
     if (iterations_out) *iterations_out = h.iterations;
     if (avg_err_out) *avg_err_out = h.last_avg;
@@ -1766,10 +1798,11 @@ int sph_iisph_solve(SphCtx *ctx, int32_t max_iterations, float omega, double eta
 int sph_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream) {
     if (!ctx || !io || nsteps < 0 || io->n_fluid < 1 || io->max_iterations < 1) return SPH_E_ARG;
     if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSharded);
     if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int s = 0; s < nsteps; ++s) {
-        int rc = single_step(ctx, st, [&] { return launch_iisph_substep(ctx, st, io, &ctx->launches); });
+        int rc = single_step(ctx, st, [&] { return launch_iisph_substep(ctx, st, io, ctx->P.n, &ctx->launches); });
         if (rc) return rc;
     }
     return SPH_OK;
@@ -1788,6 +1821,7 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) 
 int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) {
     REQUIRE_SHARD(ctx);
     if (!io || nsteps < 0 || io->n_fluid < 1) return SPH_E_ARG;
+    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphShardStep);  // sph_set_iisph sets P.dfsph too
     if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called: WCSPH contexts step with sph_shard_step");
     if (ctx->shard_bodies) return fail(ctx, SPH_E_ARG, kShardBodiesWcsph);
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
@@ -1795,7 +1829,28 @@ int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *st
         return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure: configure again");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int s = 0; s < nsteps; ++s) {
-        int rc = shard_dfsph_sequence(ctx, st, io, shard_wide(ctx), &ctx->launches);
+        int rc = shard_dfsph_sequence(ctx, st, shard_wide(ctx), &ctx->launches, [&](int64_t n_grid) {
+            return launch_dfsph_substep(ctx, st, io, n_grid, &ctx->launches);
+        });
+        if (rc) return rc;
+        ctx->shard_sequences += 1;
+    }
+    return SPH_OK;
+}
+
+int sph_shard_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream) {
+    REQUIRE_SHARD(ctx);
+    if (!io || nsteps < 0 || io->n_fluid < 1 || io->max_iterations < 1) return SPH_E_ARG;
+    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called before sph_shard_configure");
+    if (ctx->shard_bodies) return fail(ctx, SPH_E_ARG, kShardBodiesIisph);
+    if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
+    if (ctx->world != ctx->shard_world)
+        return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure: configure again");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int s = 0; s < nsteps; ++s) {
+        int rc = shard_dfsph_sequence(ctx, st, shard_wide(ctx), &ctx->launches, [&](int64_t n_grid) {
+            return launch_iisph_substep(ctx, st, io, n_grid, &ctx->launches);
+        });
         if (rc) return rc;
         ctx->shard_sequences += 1;
     }

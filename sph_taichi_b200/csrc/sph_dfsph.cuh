@@ -178,15 +178,18 @@ __global__ void k_dfsph_check(DfsphCtrl *ctrl, double n_fluid, double eta, int32
     if (ctrl->done) return;
     dfsph_check_sum(ctrl, ctrl->err, n_fluid, eta, max_iterations);
 }
-// Sharded variant: parts[r] holds rank r's error partial (this rank's own is still in ctrl->err), all-gathered over
-// the transport.  The partials are summed in RANK order, so every rank computes bit-identical avg / done / iterations
-// and issues the same number of transport calls.
+// Sharded loops: parts[r] holds rank r's error partial (this rank's own is still in ctrl->err), all-gathered over the
+// transport.  The partials are summed in RANK order, so every rank computes a bit-identical sum -- and from it the
+// same avg / done / iterations -- and issues the same number of transport calls.
+__device__ __forceinline__ double ranked_err_sum(const DfsphCtrl *ctrl, const double *parts, int32_t rank, int32_t world) {
+    double err = rank == 0 ? ctrl->err : parts[0];
+    for (int r = 1; r < world; ++r) err += r == rank ? ctrl->err : parts[r];
+    return err;
+}
 __global__ void k_dfsph_check_ranked(DfsphCtrl *ctrl, const double *parts, int32_t rank, int32_t world, double n_fluid,
                                      double eta, int32_t max_iterations) {
     if (ctrl->done) return;
-    double err = rank == 0 ? ctrl->err : parts[0];
-    for (int r = 1; r < world; ++r) err += r == rank ? ctrl->err : parts[r];
-    dfsph_check_sum(ctrl, err, n_fluid, eta, max_iterations);
+    dfsph_check_sum(ctrl, ranked_err_sum(ctrl, parts, rank, world), n_fluid, eta, max_iterations);
 }
 
 // DFSPH.py:221-227
@@ -325,7 +328,13 @@ enum {
     DX_HDR_RECV = 32,                         // the same, received from the left / right neighbour
     DX_INTS = 64
 };
-enum { DX_ALIGN = 0, DX_VELD = 1, DX_DFS = 2 };  // what a pack / unpack moves
+// what a pack / unpack moves: the alignment, or one 16-byte word per particle of one per-step array (DFSPH: veld, dfs;
+// IISPH: veld, acc = {a^p, fluid mark}, aux = {.., p / rho^2, ..})
+enum { DX_ALIGN = 0, DX_VELD = 1, DX_DFS = 2, DX_ACC = 3, DX_AUX = 4 };
+
+__device__ __forceinline__ float4 *dx_sweep_array(const DevArrays &S, int what) {
+    return what == DX_VELD ? S.veld : what == DX_DFS ? S.dfs : what == DX_ACC ? S.acc : S.aux;
+}
 
 // After k_shard_info: the ranges above, and the alignment headers.  A range longer than its message capacity is cut
 // and flagged (SPH_STATUS_HALO_CAPACITY), never written out of bounds.
@@ -366,8 +375,9 @@ __global__ void k_dfsph_shard_ranges(DevParams P, DevArrays S, int32_t *dx, int 
 }
 
 // Pack what goes to the neighbours (blockIdx.y = side: 0 = to the left, 1 = to the right) into the send staging:
-// DX_ALIGN = the 4 records of the sgw boundary layers in this rank's sorted order, DX_VELD / DX_DFS = one 16-byte word
-// per particle of the outermost owned layer.  ctrl (may be NULL): a sweep behind the converged one has nothing new.
+// DX_ALIGN = the 4 records of the sgw boundary layers in this rank's sorted order, DX_VELD / DX_DFS / DX_ACC / DX_AUX =
+// one 16-byte word per particle of the outermost owned layer.  ctrl (may be NULL): a sweep behind the converged one has
+// nothing new.
 __global__ void k_dfsph_shard_pack(DevParams P, DevArrays S, const int32_t *dx, int what, const DfsphCtrl *ctrl) {
     if (ctrl && ctrl->done) return;
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -383,7 +393,7 @@ __global__ void k_dfsph_shard_pack(DevParams P, DevArrays S, const int32_t *dx, 
         S.stage[side][2][s] = S.x0id[i];
         S.stage[side][3][s] = S.misc[i];
     } else {
-        S.stage[side][0][s] = what == DX_VELD ? S.veld[i] : S.dfs[i];
+        S.stage[side][0][s] = dx_sweep_array(S, what)[i];
     }
 }
 
@@ -393,7 +403,8 @@ __global__ void k_dfsph_shard_pack(DevParams P, DevArrays S, const int32_t *dx, 
 // inside a cell differs -- after the overwrite, ghost record begin + k IS the sender's boundary record k (cell_end stays
 // valid).  A count mismatch leaves the ghost range alone and a record of another cell is not written; both set
 // SPH_STATUS_GHOST_ALIGN.
-// DX_VELD / DX_DFS: rec[side][0] = the words of the neighbour's outermost owned layer -> this rank's first ghost layer.
+// DX_VELD / DX_DFS / DX_ACC / DX_AUX: rec[side][0] = the words of the neighbour's outermost owned layer -> this rank's
+// first ghost layer.
 __global__ void k_dfsph_shard_unpack(DevParams P, DevArrays S, int32_t *dx, int what, const DfsphCtrl *ctrl,
                                      const float4 *rec00, const float4 *rec01, const float4 *rec02, const float4 *rec03,
                                      const float4 *rec10, const float4 *rec11, const float4 *rec12, const float4 *rec13) {
@@ -406,8 +417,8 @@ __global__ void k_dfsph_shard_unpack(DevParams P, DevArrays S, int32_t *dx, int 
     const float4 *r0 = side == 0 ? rec00 : rec10;
     if (what != DX_ALIGN) {
         if (s >= e - b) return;
-        float4 *dst = what == DX_VELD ? S.veld : S.dfs;
-        dst[b + s] = r0[s];
+        SPH_EMU_CHECK(s < P.halo_cap && b + s >= 0 && b + s < P.n);
+        dx_sweep_array(S, what)[b + s] = r0[s];
         return;
     }
     const int32_t *h = dx + DX_HDR_RECV + 4 * side;

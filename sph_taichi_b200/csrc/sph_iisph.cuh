@@ -6,6 +6,10 @@
 // k_dfsph_non_pressure without cohesion, k_dfsph_predict_velocity (v* = v + dt a), k_iisph_predict (a_ii, s_i and
 // the warm start), the relaxed Jacobi loop (k_iisph_pressure_accel<false> + k_iisph_pressure_update +
 // k_iisph_check per sweep), k_iisph_pressure_accel<true> (final a^p + reactions on dynamic solids), k_iisph_advect.
+// x-slab sharded (P.slab_on, sph_shard_iisph_step): every kernel but the density pass works on the owned records; the
+// neighbours' values it reads in the first ghost layer -- v* in k_iisph_predict, aux.y = p / rho^2 in
+// k_iisph_pressure_accel, acc = {a^p, 1} in k_iisph_pressure_update -- arrive with the exchanges of the outermost owned
+// layer that the host issues after each kernel that changes them (DX_VELD, DX_AUX, DX_ACC).
 //
 // Per-step scratch, all in existing per-step workspace (no new sorted payload):
 //   dfs[i]   = {a_ii, s_i, -, -}              (the DFSPH scratch; unused in an IISPH context)
@@ -135,18 +139,31 @@ __global__ void __launch_bounds__(128) k_iisph_pressure_update(DevParams P, DevA
 
 // The loop of pressure_solve, evaluated on the device after every sweep:
 //   it = 0;  while it < max_iterations:  avg = sweep() / n_fluid;  it += 1;  if avg < eta: break
-__global__ void k_iisph_check(DfsphCtrl *ctrl, double n_fluid, double eta, int32_t max_iterations) {
-    if (ctrl->done) return;
-    const double avg = ctrl->err / n_fluid;
+// err is the sweep's whole error sum (this rank's, or the rank-ordered sum of all ranks' partials).
+__device__ __forceinline__ void iisph_check_sum(DfsphCtrl *ctrl, double err, double n_fluid, double eta,
+                                                int32_t max_iterations) {
+    const double avg = err / n_fluid;
     ctrl->last_avg = avg;
     ctrl->err = 0.0;
     ctrl->sweeps += 1;
     ctrl->iterations = ctrl->sweeps;
     if (avg < eta || ctrl->sweeps >= max_iterations) ctrl->done = 1;
 }
+__global__ void k_iisph_check(DfsphCtrl *ctrl, double n_fluid, double eta, int32_t max_iterations) {
+    if (ctrl->done) return;
+    iisph_check_sum(ctrl, ctrl->err, n_fluid, eta, max_iterations);
+}
+// Sharded: parts = the all-gathered error partials, added in rank order (ranked_err_sum), so every rank takes the same
+// decision after the same sweep.
+__global__ void k_iisph_check_ranked(DfsphCtrl *ctrl, const double *parts, int32_t rank, int32_t world, double n_fluid,
+                                     double eta, int32_t max_iterations) {
+    if (ctrl->done) return;
+    iisph_check_sum(ctrl, ranked_err_sum(ctrl, parts, rank, world), n_fluid, eta, max_iterations);
+}
 
 // advect: v += dt * acc, x += dt * v for every dynamic particle -- the fluid's acc holds a^p and its veld v*, so this
-// is v = v* + dt a^p; a dynamic solid integrates g + reactions as k_dfsph_advect does
+// is v = v* + dt a^p; a dynamic solid integrates g + reactions as k_dfsph_advect does.  Sharded: a particle that moves
+// a whole cell layer in x in one step is flagged (SPH_STATUS_SHARD_VELOCITY), as in k_dfsph_advect.
 __global__ void k_iisph_advect(DevParams P, DevArrays S) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (!dfsph_in_range(P, S, i)) return;
@@ -156,6 +173,7 @@ __global__ void k_iisph_advect(DevParams P, DevArrays S) {
     const float4 a = S.acc[i];
     v.x += P.dt * a.x; v.y += P.dt * a.y; v.z += P.dt * a.z;
     S.veld[i] = v;
+    if (P.slab_on && !(fabsf(v.x) * P.dt < P.h)) atomicOr(S.status, SPH_STATUS_SHARD_VELOCITY);
     p.x += P.dt * v.x; p.y += P.dt * v.y; p.z += P.dt * v.z;
     S.posm[i] = p;
 }

@@ -1,4 +1,4 @@
-"""x-slab sharding of one WCSPH or DFSPH scene across the GPUs of a node (one process per GPU).
+"""x-slab sharding of one WCSPH, DFSPH or IISPH scene across the GPUs of a node (one process per GPU).
 
 The reference is single-device; this is the multi-GPU extension BASELINE.json asks for (SURVEY.md section 8e).
 
@@ -34,6 +34,14 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
   eagerly, without overlap; ``SPH_SHARD_GRAPH`` does not apply.  Without the flag, and for DFSPH in any case, dynamic
   solids are refused (``STATIC_SOLIDS_ONLY`` / ``DYNAMIC_SOLIDS_WCSPH_ONLY``): the DFSPH pressure sweeps scatter the
   reactions in every sweep, which would need a reaction exchange per sweep.
+* IISPH scenes (``simulationMethod: 3``) are opt-in: ``build_sharded(..., iisph=True)`` (``run_simulation.py --gpus N
+  --shard-iisph``); without it they are refused (``IISPH_SINGLE_GPU``).  They step through ``sph_shard_iisph_step``,
+  the DFSPH step's shape with IISPH's substep: the once-per-step ghost alignment, the predicted velocities and the
+  warm-start pressures of the outermost owned layer sent once per step, and two small exchanges per relaxed Jacobi
+  sweep (its pressure accelerations, then its new pressures); the error sums are added in rank order, so every rank
+  runs the same sweeps (``last_iterations`` / ``last_avg_err``).  Fluid and static solids only: dynamic solids in
+  IISPH are refused (``DYNAMIC_SOLIDS_IISPH``).  Whether the sharded step beats one GPU at a given scene size depends
+  on the sweep count: each sweep costs two transport groups and each batch of sweeps one host wait.
 * Output: ``ShardedSimulation.dump(obj_id)`` is ``ParticleSystem.dump`` of a sharded run.  It is collective: every rank
   compacts x and v of that object's owned records on the device and rank 0 receives them over the engine's own
   transport (``sph_shard_dump``), in the global cell order of the last sort.  ``run_simulation.py --gpus N`` writes
@@ -69,9 +77,12 @@ STATUS_SOLID_SLOT = 64  # sharded with dynamic solids: two live records with one
 FLAG_FLUID, FLAG_DYNAMIC, FLAG_GHOST = 1, 2, 4  # misc.z bits of a packed record (csrc/sph_common.cuh)
 STATIC_SOLIDS_ONLY = ("x-slab sharding supports static solids only: dynamic solids (shape-matched bodies, advected "
                       "rigid blocks) are single-GPU in WCSPH and DFSPH")
-IISPH_SINGLE_GPU = "IISPH (simulationMethod 3) is single-GPU: x-slab sharding runs WCSPH (0) and DFSPH (4) scenes"
+IISPH_SINGLE_GPU = ("IISPH (simulationMethod 3) is single-GPU unless sharding is requested: x-slab sharding of an "
+                    "IISPH scene is opt-in (build_sharded(..., iisph=True), run_simulation.py --gpus N --shard-iisph)")
 DYNAMIC_SOLIDS_WCSPH_ONLY = ("x-slab sharding of dynamic solids is WCSPH only: the DFSPH pressure sweeps scatter the "
                              "reactions onto the bodies in every sweep, which would need a reaction exchange per sweep")
+DYNAMIC_SOLIDS_IISPH = ("x-slab sharding of dynamic solids is WCSPH only: dynamic solids in IISPH scenes are single-GPU "
+                        "(sharded IISPH runs fluid and static solids)")
 
 
 def scene_params(cfg):
@@ -264,8 +275,9 @@ class ShardedSimulation:
         from . import engine as _engine
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dfsph = cfg.get_cfg("simulationMethod") == 4
-        if self.dfsph and not n_fluid:
-            raise ValueError("a sharded DFSPH scene needs n_fluid, the fluid particle count of ALL ranks")
+        self.iisph = cfg.get_cfg("simulationMethod") == 3
+        if (self.dfsph or self.iisph) and not n_fluid:
+            raise ValueError("a sharded DFSPH or IISPH scene needs n_fluid, the fluid particle count of ALL ranks")
         self.device = torch.device(device)
         self.slabs0 = [tuple(int(v) for v in s_) for s_ in slabs]
         ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
@@ -277,16 +289,23 @@ class ShardedSimulation:
         self.bodies = None if bodies is None else list(bodies)
         if self.bodies is not None and self.dfsph:
             raise NotImplementedError(DYNAMIC_SOLIDS_WCSPH_ONLY)
+        if self.bodies is not None and self.iisph:
+            raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
         self.eng = _engine.Engine(scene_params(cfg), n_max=self.n_cap, n_solid=self.n_solid,
                                   n_bodies=len(self.bodies or []), device=self.device)
         e = self.eng
         self._load(mine, n_mine, uniform_hint)
         self.last_iterations_v = self.last_iterations = 0
         self._io = None
+        self.last_avg_err = 0.0
         if self.dfsph:
             e.set_dfsph(True)
             from .DFSPH import dfsph_step_io
             self._io = dfsph_step_io(float(cfg.get_cfg("timeStepSize")), float(cfg.get_cfg("density0")), n_fluid)
+        elif self.iisph:
+            e.set_iisph(True)  # before sph_shard_configure: the library refuses it on a sharded context
+            from .IISPH import iisph_step_io
+            self._io = iisph_step_io(n_fluid)
         # ---- transport: NCCL inside the library (its own communicator), or a caller-supplied one (tests) ----
         if transport is not None:
             self._transport = transport
@@ -337,14 +356,19 @@ class ShardedSimulation:
     # ---- stepping --------------------------------------------------------------------------------------
     def step(self, n=1):
         """``n`` sharded steps.  DFSPH: ``last_iterations_v`` / ``last_iterations`` (and ``last_avg_err_v`` /
-        ``last_avg_err``) are those of the last step, the same on every rank; the call waits on the device once per
-        batch of Jacobi sweeps."""
+        ``last_avg_err``) are those of the last step, the same on every rank; IISPH: ``last_iterations`` /
+        ``last_avg_err`` (pressure sweeps and their last average error), the same on every rank.  Both wait on the
+        device once per batch of Jacobi sweeps."""
         e = self.eng
         if self.dfsph:
             io = self._io
             e._check(e.lib.sph_shard_dfsph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_dfsph_step")
             self.last_iterations_v, self.last_iterations = int(io.iterations_v), int(io.iterations)
             self.last_avg_err_v, self.last_avg_err = float(io.avg_err_v), float(io.avg_err)
+        elif self.iisph:
+            io = self._io  # first_batch: in, the previous step's sweeps; out, this step's
+            e._check(e.lib.sph_shard_iisph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_iisph_step")
+            self.last_iterations, self.last_avg_err = int(io.iterations), float(io.avg_err)
         else:
             e._check(e.lib.sph_shard_step(e.ctx, int(n), e._stream()), "sph_shard_step")
         self.steps_done += int(n)
@@ -475,19 +499,27 @@ class ShardedSimulation:
 
 
 def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1.2, rebalance_every=8, slabs=None,
-                  transport=None, dynamic_solids=False):
+                  transport=None, dynamic_solids=False, iisph=False):
     """Assemble the scene on every rank, plan the slabs from the initial layer histogram and load this rank's
     share into a CUDA engine.  ``dynamic_solids=True`` opts in to sharding WCSPH scenes with dynamic solids
     (3 ghost layers, reactions gathered across cuts, bodies solved on every rank from an all-gather of their particles).
+    ``iisph=True`` opts in to sharding an IISPH scene (fluid and static solids).
     Returns (ShardedSimulation, n_total)."""
     from .config_builder import SimConfig
     from .scene import assemble_particles
 
     cfg = SimConfig(scene_dict)
     method = cfg.get_cfg("simulationMethod")
-    if method not in (0, 4):
-        raise NotImplementedError(IISPH_SINGLE_GPU if method == 3 else
-                                  f"x-slab sharding runs WCSPH (0) and DFSPH (4) scenes, not simulationMethod {method}")
+    if method == 3 and not iisph:
+        raise NotImplementedError(IISPH_SINGLE_GPU)
+    if method not in (0, 3, 4):
+        raise NotImplementedError(f"x-slab sharding runs WCSPH (0), DFSPH (4) and IISPH (3) scenes, not "
+                                  f"simulationMethod {method}")
+    if iisph and method != 3:
+        raise ValueError(f"iisph=True shards an IISPH scene (simulationMethod 3), not simulationMethod {method}")
+    if iisph and (dynamic_solids or any(o.get("isDynamic") for o in
+                                        list(cfg.get_rigid_bodies() or []) + list(cfg.get_rigid_blocks() or []))):
+        raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
     radius = cfg.get_cfg("particleRadius")
     h = radius * 4.0
     arrays, object_collection, _, counts = assemble_particles(cfg, 3, 2 * radius)

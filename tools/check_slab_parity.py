@@ -14,6 +14,15 @@ with the single engine's, checks that every rank reported bit-identical counts a
 that after the last step's ghost alignment each ghost record holds the x_0 of the neighbour's boundary record at the
 same position.
 
+--iisph runs the scene with the IISPH solver (dt = 1e-3, build_sharded(iisph=True)) and checks the same things as
+--dfsph: the pressure sweep count of every step against the single engine's, counts and average errors bit-identical
+across ranks in every step, and the ghost alignment; it also reports the per-step average errors of both engines.  The
+tolerance rule is test_iisph_steps_vs_oracle's: |dx| / d < 2e-3 when the sweep counts match, 5e-2 otherwise.
+
+--collide splits the fluid into two blocks (objects 0 and 1) that move toward each other at +-vx and meet at the
+initial cut of a balanced two-rank start: the fluid along the contact plane is compressed above the rest density within
+a few steps, so the pressure solves of DFSPH and IISPH run several sweeps right at the cut.
+
 --dynamic-body / --dynamic-block add dynamic solids (WCSPH, build_sharded(dynamic_solids=True)): a shape-matched cube
 (tests/golden/cube.obj) straddling the fluid's x fraction 1/world (1/2 on one rank) -- the initial cut of a balanced
 start -- and resting on the fluid surface, and an advected dynamic rigid block on the surface at 3/4 of the fluid.  The tool then also reports whether
@@ -51,6 +60,18 @@ def static_block_scene(c, d):
     sc["RigidBlocks"] = [{"objectId": 1, "start": lo, "end": [s + (k - 0.5) * d for s, k in zip(lo, n)],
                           "translation": [0.0, 0.0, 0.0], "scale": [1, 1, 1], "velocity": [0.0, 0.0, 0.0],
                           "density": 1000.0, "color": [255, 255, 255], "isDynamic": False}]
+    return sc
+
+
+def colliding_blocks_scene(c, d, vx):
+    """The dam break of ``c`` particles split in x into two blocks one lattice spacing apart, the left half (object 0)
+    moving at +vx, the right half (object 1) at -vx (--collide)."""
+    sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12], start=[0.06] * 3)
+    left = sc["FluidBlocks"][0]
+    half = c[0] // 2
+    right = dict(left, objectId=1, start=[0.06 + half * d] + left["start"][1:], velocity=[-vx, 0.0, 0.0])
+    left.update(end=[0.06 + (half - 0.5) * d] + left["end"][1:], velocity=[vx, 0.0, 0.0])
+    sc["FluidBlocks"].append(right)
     return sc
 
 
@@ -93,13 +114,17 @@ def main():
     ap.add_argument("--skew", type=int, default=0, help="shift every interior slab cut by this many layers at the start")
     ap.add_argument("--rebalance-every", type=int, default=8)
     ap.add_argument("--dfsph", action="store_true", help="DFSPH instead of WCSPH (simulationMethod 4, dt = 4e-3)")
+    ap.add_argument("--iisph", action="store_true",
+                    help="IISPH instead of WCSPH (simulationMethod 3, dt = 1e-3; build_sharded(iisph=True))")
     ap.add_argument("--static-block", action="store_true",
                     help="the fluid rests on a static rigid block that straddles every cut (static_block_scene)")
+    ap.add_argument("--collide", action="store_true",
+                    help="two fluid blocks meeting at +-vx at the initial cut (colliding_blocks_scene)")
     ap.add_argument("--dynamic-body", action="store_true", help="a shape-matched cube across the initial cut (WCSPH)")
     ap.add_argument("--dynamic-block", action="store_true", help="an advected dynamic rigid block (WCSPH)")
     ap.add_argument("--scene", default=None, choices=sorted(scene.NAMED_SCENES),
                     help="a named scene as it is (--counts, --vx and --static-block do not apply; a DFSPH scene needs "
-                         "--dfsph for the iteration-count comparison)")
+                         "--dfsph for the iteration-count comparison, an IISPH scene --iisph)")
     ap.add_argument("--soak", type=int, default=0, metavar="EVERY",
                     help="long run: read the step state (capacity / out-of-grid flags raise) every EVERY steps; the "
                          "flow is chaotic over thousands of steps, so the verdict is the particle set, finiteness and "
@@ -121,6 +146,8 @@ def main():
         d = 2.0 * sc["Configuration"]["particleRadius"]
     elif a.static_block:
         sc = static_block_scene(c, d)
+    elif a.collide:
+        sc = colliding_blocks_scene(c, d, a.vx)
     else:
         sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12], start=[0.06] * 3)
     dynamic = a.dynamic_body or a.dynamic_block
@@ -128,10 +155,13 @@ def main():
         sc = add_dynamic_solids(sc, c, d, world, a.dynamic_body, a.dynamic_block)
     if a.scene and any(b.get("isDynamic") for b in sc.get("RigidBodies", []) + sc.get("RigidBlocks", [])):
         dynamic = True
-    if not a.scene:
+    if not a.scene and not a.collide:
         sc["FluidBlocks"][0]["velocity"] = [a.vx, 0.0, 0.0]
     if a.dfsph and sc["Configuration"]["simulationMethod"] != 4:
         sc = scene._as_dfsph(sc)
+    if a.iisph and sc["Configuration"]["simulationMethod"] != 3:
+        sc = scene._as_iisph(sc)
+    jacobi = a.dfsph or a.iisph  # one step per call, sweep counts and the ghost alignment checked
     transport = slab.GlooTransport() if (EMU and world > 1) else None
     slabs = None
     if a.skew:  # deliberately unbalanced start: every interior cut shifted, the balancer has to move them back
@@ -145,7 +175,7 @@ def main():
         cuts = [cuts[0]] + [c_ + a.skew for c_ in cuts[1:-1]] + [cuts[-1]]
         slabs = [(cuts[r], cuts[r + 1]) for r in range(world)]
     sim, n_total = slab.build_sharded(sc, rank, world, dev, rebalance_every=a.rebalance_every, slabs=slabs,
-                                      transport=transport, dynamic_solids=dynamic)
+                                      transport=transport, dynamic_solids=dynamic, iisph=a.iisph)
     first = sim.info()
     trace = []
     if a.soak:
@@ -160,6 +190,10 @@ def main():
         for _ in range(a.steps):  # one step per call: the iteration counts of every step
             sim.step(1)
             trace.append((sim.last_iterations_v, sim.last_iterations, sim.last_avg_err_v.hex(), sim.last_avg_err.hex()))
+    elif a.iisph:
+        for _ in range(a.steps):  # one step per call: the sweep counts of every step
+            sim.step(1)
+            trace.append((sim.last_iterations, sim.last_avg_err.hex()))
     elif dynamic:
         for _ in range(a.steps):  # one step per call: the body states of every step
             sim.step(1)
@@ -171,7 +205,7 @@ def main():
     gathered = slab.gather_owned(sim)
     meta = {"owned": (first["owned"], last["owned"]), "halo": 64 * last["halo_records_sent"], "trace": trace,
             "slab0": (first["x_lo"], first["x_hi"]), "slab1": (last["x_lo"], last["x_hi"])}
-    if a.dfsph:
+    if jacobi:
         # the x_0 of the ghost layers ([0, own_begin) and [own_end, n_live)) and of the owned records, as the last
         # step's alignment left them (advect and clamp touch owned records only; the sort comes with the next step)
         x0 = sim.record_views()[2][:, :3].cpu().numpy()
@@ -192,17 +226,25 @@ def main():
     if rank == 0:
         ps = ParticleSystem(SimConfig(sc), device=dev)
         s = ps.build_solver(); s.initialize()
-        single_counts = []
+        single_counts, single_errs = [], []
         if a.dfsph:
             for _ in range(a.steps):
                 s.step(1)
                 single_counts.append([s.last_iterations_v, s.last_iterations])
+        elif a.iisph:
+            for _ in range(a.steps):
+                s.step(1)
+                single_counts.append([s.last_iterations])
+                single_errs.append(float(s.last_avg_density_error))
         else:
             s.step(a.steps)
         bodies = None
         if dynamic:
             bodies = {oid: sim.body_state(b) for b, (oid, *_rest) in enumerate(sim.bodies)}
         cmp_ = slab.compare_with_single(gathered, ps, d, bodies=bodies)
+        lo_, hi_ = (torch.tensor(sc["Configuration"][k], dtype=torch.float32) for k in ("domainStart", "domainEnd"))
+        X_ = gathered[0].cpu()
+        cmp_["finite_inside_domain"] = bool(torch.isfinite(X_).all() and (X_ >= lo_).all() and (X_ <= hi_).all())
         X0, OID0 = gathered[2], gathered[3]
         migrated = any(m["owned"][0] != m["owned"][1] for m in metas)
         moved = any(tuple(m["slab0"]) != tuple(m["slab1"]) for m in metas)
@@ -214,8 +256,8 @@ def main():
         if a.dynamic_body and not a.scene:  # [first, last + 1) cell layer the cube occupies at the start
             lay = slab.layer_of(np.asarray(X0[OID0 == 2].cpu().numpy()), 2 * d)
             cmp_["body_layers"] = [int(lay.min()), int(lay.max()) + 1]
-        if a.dfsph:
-            counts = [list(t[:2]) for t in metas[0]["trace"]]
+        if jacobi:
+            counts = [list(t[:2 if a.dfsph else 1]) for t in metas[0]["trace"]]
             same_on_ranks = all([list(t) for t in m["trace"]] == [list(t) for t in metas[0]["trace"]] for m in metas)
             aligned = True
             for r in range(1, world):  # rank r's left ghosts <-> rank r-1's last owned records, and vice versa
@@ -224,7 +266,8 @@ def main():
                 aligned = aligned and gl == metas[r - 1]["x0_owned"][len(metas[r - 1]["x0_owned"]) - len(gl):]
                 aligned = aligned and gr == metas[r]["x0_owned"][:len(gr)]
             counts_match = counts == single_counts
-            # the rule of test_dfsph_steps_vs_oracle: tight when the solvers ran the same sweeps
+            # the rule of test_dfsph_steps_vs_oracle / test_iisph_steps_vs_oracle: tight when the solvers ran the same
+            # sweeps
             tol = 2e-3 if counts_match else 5e-2
             ok = (cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < tol and same_on_ranks and aligned
                   and slab.static_solids_ok(cmp_))
@@ -232,6 +275,8 @@ def main():
                         bit_identical_across_ranks=same_on_ranks, ghosts_aligned=aligned,
                         transport_groups=[m["transport"][0] for m in metas],
                         transport_bytes=[m["transport"][1] for m in metas])
+            if a.iisph:
+                cmp_.update(avg_err_sharded=[float.fromhex(t[1]) for t in metas[0]["trace"]], avg_err_single=single_errs)
         if dynamic:
             same_on_ranks = all(m["trace"] == metas[0]["trace"] for m in metas)
             g_y, t = float(sc["Configuration"]["gravitation"][1]), a.steps * float(sc["Configuration"]["timeStepSize"])
