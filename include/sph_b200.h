@@ -200,7 +200,7 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
  * deviations from IISPH.py are listed there).  sph_set_iisph(1) puts a context in IISPH mode: the density pass has
  * DFSPH semantics (no clamp, no EOS), and the WCSPH / DFSPH calls (sph_step, sph_dfsph_*, sph_shard_step,
  * sph_shard_profile_step, sph_shard_dfsph_step) and sph_shard_configure_bodies refuse the context (dynamic solids in
- * IISPH are single-GPU); sph_set_dfsph or sph_set_iisph(0) leave the mode (the context is then a WCSPH one unless
+ * IISPH shard through sph_shard_configure_iisph_bodies only); sph_set_dfsph or sph_set_iisph(0) leave the mode (the context is then a WCSPH one unless
  * sph_set_dfsph(1) follows; sph_set_iisph(0) on a context that is not in IISPH mode changes nothing).  An IISPH context
  * may be x-slab sharded: sph_set_iisph(1) BEFORE sph_shard_configure (it is refused on a sharded context), then
  * sph_shard_iisph_step (below).  The IISPH calls refuse a context that is not in IISPH mode, and sph_iisph_op,
@@ -254,8 +254,8 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream);
  * rides the exchange like a fluid one (posm.w = its boundary volume m_V, misc = material, flags, solid_id) and is
  * staged unchanged, so the caller must pack every solid with its final start-up m_V -- the value the single engine's
  * sph_boundary_volume computes over the WHOLE scene (a solid's neighbours may sit across a cut).  Dynamic solids
- * (shape-matched bodies, advected rigid blocks) shard in WCSPH only through sph_shard_configure_bodies (below);
- * sph_shard_configure refuses them, and on a sharded
+ * (shape-matched bodies, advected rigid blocks) shard only through sph_shard_configure_bodies (WCSPH) and
+ * sph_shard_configure_iisph_bodies (IISPH), both below; in DFSPH they are single-GPU.  sph_shard_configure refuses them, and on a sharded
  * context sph_set_solid_count refuses the dynamic flag, sph_set_rigid_bodies a body table, and sph_boundary_volume,
  * sph_compute_com, sph_compute_rigid_rest_cm and sph_solve_constraints refuse to run (they walk solid ids through a
  * slot map that migration leaves stale for solids of other ranks).
@@ -270,7 +270,8 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream);
  * IISPH contexts (sph_set_iisph(1) before sph_shard_configure; fluid + static solids) step with sph_shard_iisph_step:
  * the same step shape as sph_shard_dfsph_step, with the outermost owned layer's v* sent after predict_velocity, its
  * aux word (p / rho^2) after the diagonal / source pass and after every pressure update, and its acc word (a^p) after
- * every pressure-acceleration pass -- two exchanges per relaxed Jacobi sweep.
+ * every pressure-acceleration pass -- two exchanges per relaxed Jacobi sweep.  With dynamic solids
+ * (sph_shard_configure_iisph_bodies) one more word follows the loop: the final pressures (misc.y).
  *
  * The exchange goes through an SphTransport: NCCL point-to-point (libnccl.so.2 is dlopen'ed; the communicator
  * belongs to this library, created from an id the caller distributes), or caller-supplied functions (the CPU
@@ -307,6 +308,23 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
  * sph_shard_profile_step and sph_shard_dfsph_step are refused on such a context. */
 int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                                int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies);
+/* Opt-in sharding of IISPH scenes with DYNAMIC solids: the arguments, checks and layout of sph_shard_configure_bodies
+ * (ghost_layers >= 3, the whole scene's body table with rest_cm), on a context in IISPH mode -- sph_set_iisph(1) must
+ * have been called before it; WCSPH and DFSPH contexts are refused.  IISPH scatters the rigid reactions once per step,
+ * after the pressure loop, so no per-sweep reaction exchange is needed.  sph_shard_iisph_step then runs
+ *     plan -> classify + sort -> info -> DX ranges -> ghost alignment (3 layers) -> solid-id slot map -> moving
+ *     boundary volumes (owned layers + ghost layers 1-2) -> the IISPH substep of sph_shard_iisph_step, whose final
+ *     pressure acceleration does NOT scatter reactions -> [misc: the final pressures] -> the reactions GATHERED onto
+ *     each owned dynamic solid (fluid of the owned layers and ghost layer 1) -> advect -> body records -> all-gather
+ *     -> shape matching on every rank, and clamps -> fluid wall clamp -> the record exchange.
+ * Only the summation order of the reactions differs from sph_iisph_step.  cm and R are bit-identical on every rank.
+ * Transport groups per step: alignment, v*, warm-start aux, two per sweep launched, the final pressures, the body
+ * all-gather (world > 1 and a non-empty body table), the record exchange.  The refusals of a
+ * sph_shard_configure_bodies context apply (body table fixed, solid-id calls, sph_shard_step, sph_shard_profile_step,
+ * sph_shard_dfsph_step, the single-GPU IISPH calls). */
+int sph_shard_configure_iisph_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers,
+                                     int64_t halo_capacity, int32_t rebalance_every, const SphRigidBody *bodies,
+                                     int32_t n_bodies);
 /* first sort of the packed particles + the first halo exchange (no physics) */
 int sph_shard_begin(SphCtx *ctx, void *stream);
 /* nsteps sharded SPHBase.step()s (sph_base.py:263-271): asynchronous launches that run ahead of the device (no host
@@ -319,7 +337,8 @@ int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream);
  * moves a whole cell layer in x in one step sets SPH_STATUS_SHARD_VELOCITY (the record exchange would lose it);
  * sph_shard_info reports the status word. */
 int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream);
-/* nsteps sharded IISPH SPHBase.step()s of an IISPH context (fluid + static solids): the step of sph_iisph_step with
+/* nsteps sharded IISPH SPHBase.step()s of an IISPH context (fluid + static solids; with dynamic solids on a context
+ * configured by sph_shard_configure_iisph_bodies, whose additions to the order below are listed there): the step of sph_iisph_step with
  * `io` used the same way, except that io->n_fluid is the GLOBAL fluid count (all ranks).  One step:
  *     plan -> classify + sort -> info -> DX ranges -> ghost alignment -> densities (owned + first ghost layer)
  *     -> non-pressure forces -> predict velocity -> [v*] -> diagonal, source, warm start -> [aux]

@@ -13,7 +13,8 @@ the ASCII PLY export of object 0 (`exportPly`) are kept.  Extra flags: --frames,
 The loop and the output files are those of the single-GPU run; rank 0 writes them (`ShardedSimulation.dump`
 gathers object 0 over the engine's own transport; the torch process group, gloo, only carries the NCCL id).
 `--gpus 1` runs the sharded engine on one GPU without torch.distributed.run.  IISPH scenes (simulationMethod 3) shard
-only on request, `--gpus N --shard-iisph`; without the flag they are refused.
+only on request, `--gpus N --shard-iisph`; without the flag they are refused.  IISPH scenes with dynamic solids need
+`--gpus N --shard-iisph-bodies` (which implies `--shard-iisph`).
 """
 import argparse
 import copy
@@ -98,12 +99,13 @@ def _resolved_scene(config):
     return sc
 
 
-def run_sharded(config, scene_name, frames, device, transport=None, quiet=False, iisph=False):
+def run_sharded(config, scene_name, frames, device, transport=None, quiet=False, iisph=False, iisph_bodies=False):
     """The same loop and output files as `run_single`, on the x-slab sharded engine: this process is rank RANK of
     WORLD_SIZE (environment, default 0 of 1) on `device`.  Every rank steps and joins each `dump`; rank 0 writes the
     files and prints the summary.  `transport`: an SphTransport object in place of the library's NCCL communicator
     (slab.GlooTransport); with world > 1 and no transport the torch process group must be initialised.  `iisph`:
-    shard an IISPH scene (`slab.build_sharded(..., iisph=True)`)."""
+    shard an IISPH scene (`slab.build_sharded(..., iisph=True)`); `iisph_bodies`: one with dynamic solids
+    (`iisph_bodies=True`)."""
     from sph_taichi_b200 import slab
     from sph_taichi_b200.sph_base import posed_mesh
 
@@ -112,7 +114,7 @@ def run_sharded(config, scene_name, frames, device, transport=None, quiet=False,
     dynamic = any(o.get("isDynamic") for o in list(config.get_rigid_bodies()) + list(config.get_rigid_blocks()))
     try:
         sim, n_total = slab.build_sharded(_resolved_scene(config), rank, world, device, transport=transport,
-                                          dynamic_solids=dynamic, iisph=iisph)
+                                          dynamic_solids=dynamic, iisph=iisph, iisph_bodies=iisph_bodies)
     except NotImplementedError as exc:
         raise SystemExit(f"{scene_name}: {exc}") from exc
     substeps = config.get_cfg("numberOfStepsPerRenderUpdate")
@@ -171,7 +173,8 @@ def main_sharded(args, config, scene_name):
         os.environ.setdefault("MASTER_PORT", "29511")
         dist.init_process_group("gloo", rank=rank, world_size=world)  # carries the NCCL id only
     try:
-        return run_sharded(config, scene_name, args.frames, dev, quiet=args.quiet, iisph=args.shard_iisph)
+        return run_sharded(config, scene_name, args.frames, dev, quiet=args.quiet, iisph=args.shard_iisph,
+                           iisph_bodies=args.shard_iisph_bodies)
     finally:
         if world > 1:
             dist.destroy_process_group()
@@ -188,7 +191,11 @@ if __name__ == "__main__":
                         help="x-slab sharded run on N GPUs, one process per GPU (N > 1: under torch.distributed.run)")
     parser.add_argument("--shard-iisph", action="store_true",
                         help="with --gpus: shard an IISPH scene (simulationMethod 3; fluid and static solids)")
+    parser.add_argument("--shard-iisph-bodies", action="store_true",
+                        help="with --gpus: shard an IISPH scene with dynamic solids (implies --shard-iisph)")
     args = parser.parse_args()
+    if args.shard_iisph_bodies and args.gpus is None:
+        parser.error("--shard-iisph-bodies needs --gpus N")
     if args.shard_iisph and args.gpus is None:
         parser.error("--shard-iisph needs --gpus N")
     if args.scene:

@@ -28,7 +28,7 @@ ABI_SYMBOLS = [
     "sph_comm_unique_id", "sph_comm_init_nccl", "sph_comm_set_transport", "sph_shard_configure", "sph_shard_begin",
     "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step", "sph_shard_dfsph_step",
     "sph_shard_transport_stats", "sph_shard_configure_bodies", "sph_shard_dump", "sph_set_iisph", "sph_iisph_op",
-    "sph_iisph_solve", "sph_iisph_step", "sph_iisph_read", "sph_shard_iisph_step",
+    "sph_iisph_solve", "sph_iisph_step", "sph_iisph_read", "sph_shard_iisph_step", "sph_shard_configure_iisph_bodies",
 ]
 
 
@@ -160,6 +160,7 @@ def load():
         "sph_comm_set_transport": (C.c_int, [vp, C.POINTER(SphTransport), i32, i32]),
         "sph_shard_configure": (C.c_int, [vp, i32, i32, i32, i64, i32]),
         "sph_shard_configure_bodies": (C.c_int, [vp, i32, i32, i32, i64, i32, C.POINTER(SphRigidBody), i32]),
+        "sph_shard_configure_iisph_bodies": (C.c_int, [vp, i32, i32, i32, i64, i32, C.POINTER(SphRigidBody), i32]),
         "sph_shard_begin": (C.c_int, [vp, vp]),
         "sph_shard_step": (C.c_int, [vp, i32, vp]),
         "sph_halo_exchange": (C.c_int, [vp, vp]),

@@ -39,7 +39,11 @@ const char *const kIisphShardStep =
     "this context is in IISPH mode (sph_set_iisph): a sharded IISPH context steps with sph_shard_iisph_step";
 const char *const kIisphAfterConfigure = "call sph_set_iisph(1) before sph_shard_configure, not on a sharded context";
 const char *const kShardBodiesIisph =
-    "x-slab sharding of dynamic solids is WCSPH only: dynamic solids in IISPH are single-GPU";
+    "x-slab sharding of dynamic solids is WCSPH only: dynamic solids in IISPH are single-GPU unless requested: "
+    "sph_shard_configure_iisph_bodies";
+const char *const kShardIisphBodiesContext =
+    "sph_shard_configure_iisph_bodies shards the dynamic solids of an IISPH context: call sph_set_iisph(1) before it "
+    "(WCSPH contexts use sph_shard_configure_bodies; dynamic solids in DFSPH are single-GPU)";
 const char *const kShardBodiesFixed =
     "the body table of a context configured by sph_shard_configure_bodies is fixed: configure a new context";
 
@@ -208,7 +212,9 @@ struct SphCtx {
     // sharded DFSPH: records per side of the ghost alignment (sgw layers) and of a per-sweep exchange (one layer)
     int32_t align_cap = 0, sweep_cap = 0;
     int shard_world = 1;  // world size the shard buffer's per-rank error partials were sized for
-    bool shard_bodies = false;  // configured by sph_shard_configure_bodies: steps with shard_bodies_sequence
+    // configured by sph_shard_configure_bodies (WCSPH: steps with shard_bodies_sequence) or
+    // sph_shard_configure_iisph_bodies (IISPH: shard_dfsph_sequence with its body hooks)
+    bool shard_bodies = false;
     uint64_t xfer_groups = 0, xfer_bytes = 0;  // transport groups issued from the host, and the bytes this rank sent
     // sph_shard_dump's device scratch (library-owned, grown on demand): the header sent, the headers received, the
     // tile counts
@@ -936,6 +942,54 @@ inline int64_t body_particles(const std::vector<SphRigidBody> &bodies) {
     return n;
 }
 
+// Sharded steps with dynamic solids, after the sort (and, in the Jacobi solvers' step, after the ghost alignment, which
+// reorders records inside cells): the solid-id slot map of the live records, then the moving boundary volumes of the
+// owned layers and ghost layers 1-2.
+int launch_shard_solid_slots(SphCtx *c, cudaStream_t st, int64_t *kernels) {
+    const DevParams &P = c->P;
+    if (P.n_solid == 0) return SPH_OK;
+    // k_rank_move also wrote the slots of trash records: only the live ones may be walked
+    CUDA_TRY(c, cudaMemsetAsync(c->S.solid_slot, 0xff, (size_t)P.n_solid * 4, st));
+    k_shard_solid_slots<<<step_grid(c, P.n, 256, 8), 256, 0, st>>>(P, c->S);
+    *kernels += 1;
+    if (c->has_dynamic_solids) {
+        k_boundary_volume<true><<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S, /*moving=*/1);
+        *kernels += 1;
+    }
+    return SPH_OK;
+}
+
+// solve_rigid_body of a sharded step: k_rigid's solve on every rank from the records of all body particles, gathered in
+// one transport group, then the clamps of the dynamic solids outside every body.
+int launch_shard_body_solve(SphCtx *c, cudaStream_t st, int64_t *kernels) {
+    const DevParams &P = c->P;
+    const int nb = (int)c->bodies.size();
+    if (nb == 0) return SPH_OK;
+    const int64_t n_rec = body_particles(c->bodies);
+    float4 *tables = shard_body_tables(c);
+    float4 *mine = tables + 2 * (size_t)c->rank * n_rec;
+    k_shard_body_pack<<<nb, 256, 0, st>>>(P, c->S, dev_bodies(c), mine);
+    *kernels += 1;
+    CUDA_TRY(c, cudaGetLastError());
+    if (c->world > 1) {
+        const uint64_t bytes = (uint64_t)n_rec * 32;
+        int rc = transport_group(
+            c, st, [](int, int) { return SPH_OK; },
+            [&] {
+                for (int r = 0; r < c->world; ++r) {
+                    if (r == c->rank) continue;
+                    if (int rc2 = xfer_pair(c, st, r, mine, tables + 2 * (size_t)r * n_rec, bytes)) return rc2;
+                }
+                return SPH_OK;
+            });
+        if (rc) return rc;
+    }
+    k_shard_body_solve<<<nb, RIGID_THREADS, 0, st>>>(P, c->S, dev_bodies(c), nb, tables, (int)n_rec, c->world);
+    k_enforce_boundary_solid<true><<<blocks_for(P.n_solid, 256), 256, 0, st>>>(P, c->S, nb, dev_bodies(c), nb);
+    *kernels += 2;
+    return SPH_OK;
+}
+
 // One sharded WCSPH SPHBase.step() with dynamic solids (sph_shard_configure_bodies), in the order of launch_step +
 // launch_rigid_solve, on one stream and without overlap:
 //   plan -> classify + sort -> info -> solid-id slot map -> moving boundary volumes (owned + ghost layers 1-2)
@@ -951,51 +1005,19 @@ int shard_bodies_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernel
     const DevParams &P = c->P;
     k_shard_info<<<1, 32, 0, st>>>(P, c->S, P.sgw + (wide ? 2 : 1), wide ? P.halo_cap : c->narrow_cap);
     *kernels += 1;
-    if (P.n_solid > 0) {
-        // k_rank_move also wrote the slots of trash records: only the live ones may be walked
-        CUDA_TRY(c, cudaMemsetAsync(c->S.solid_slot, 0xff, (size_t)P.n_solid * 4, st));
-        k_shard_solid_slots<<<step_grid(c, P.n, 256, 8), 256, 0, st>>>(P, c->S);
-        *kernels += 1;
-        if (c->has_dynamic_solids) {
-            k_boundary_volume<true><<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S, /*moving=*/1);
-            *kernels += 1;
-        }
-    }
+    rc = launch_shard_solid_slots(c, st, kernels);
+    if (rc) return rc;
     launch_pair_density(c, st, kernels, /*split_mode=*/0);
     PDL_LAUNCH((k_force_packed<FORCE_BATCH, FORCE_THREADS, true>), blocks_for(P.n, FORCE_THREADS), FORCE_THREADS, st,
                P, c->S, 0);
     *kernels += 1;
     CUDA_TRY(c, cudaGetLastError());
-    const int nb = (int)c->bodies.size();
     if (P.n_solid > 0) {
         k_shard_reactions<<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S);
         *kernels += 1;
     }
-    if (nb > 0) {
-        // k_rigid's solve on every rank: the records of all body particles, gathered, in one transport group
-        const int64_t n_rec = body_particles(c->bodies);
-        float4 *tables = shard_body_tables(c);
-        float4 *mine = tables + 2 * (size_t)c->rank * n_rec;
-        k_shard_body_pack<<<nb, 256, 0, st>>>(P, c->S, dev_bodies(c), mine);
-        *kernels += 1;
-        CUDA_TRY(c, cudaGetLastError());
-        if (c->world > 1) {
-            const uint64_t bytes = (uint64_t)n_rec * 32;
-            rc = transport_group(
-                c, st, [](int, int) { return SPH_OK; },
-                [&] {
-                    for (int r = 0; r < c->world; ++r) {
-                        if (r == c->rank) continue;
-                        if (int rc2 = xfer_pair(c, st, r, mine, tables + 2 * (size_t)r * n_rec, bytes)) return rc2;
-                    }
-                    return SPH_OK;
-                });
-            if (rc) return rc;
-        }
-        k_shard_body_solve<<<nb, RIGID_THREADS, 0, st>>>(P, c->S, dev_bodies(c), nb, tables, (int)n_rec, c->world);
-        k_enforce_boundary_solid<true><<<blocks_for(P.n_solid, 256), 256, 0, st>>>(P, c->S, nb, dev_bodies(c), nb);
-        *kernels += 2;
-    }
+    rc = launch_shard_body_solve(c, st, kernels);
+    if (rc) return rc;
     k_shard_apply<<<dim3(blocks_for(P.halo_cap, 256), 2), 256, 0, st>>>(P, c->S, /*copy_all=*/1);
     *kernels += 1;
     CUDA_TRY(c, cudaGetLastError());
@@ -1112,19 +1134,19 @@ int shard_setup(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, i
     return SPH_OK;
 }
 
-}  // namespace
-extern "C" {
-
-int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
-                               int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
+// sph_shard_configure_bodies (iisph = false: a WCSPH context) and sph_shard_configure_iisph_bodies (iisph = true: an
+// IISPH context): the same checks and set-up, only the solver asked for differs.
+int shard_configure_bodies(SphCtx *ctx, bool iisph, int32_t x_lo, int32_t x_hi, int32_t ghost_layers,
+                           int64_t halo_capacity, int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
     if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kShardBodiesIisph);
+    if (!iisph && ctx->iisph) return fail(ctx, SPH_E_ARG, kShardBodiesIisph);
+    if (iisph && !ctx->iisph) return fail(ctx, SPH_E_ARG, kShardIisphBodiesContext);
     if (x_lo < 0 || x_hi > ctx->P.gx || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
     if (ghost_layers < 3)
         return fail(ctx, SPH_E_ARG, "dynamic solids need ghost_layers >= 3: the moving boundary volumes of the second "
                                     "ghost layer (read by the first layer's densities) sum solids of the third");
-    if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, kShardBodiesWcsph);
+    if (!iisph && ctx->P.dfsph) return fail(ctx, SPH_E_ARG, kShardBodiesWcsph);
     if (!ctx->P.uniform_fluid)
         return fail(ctx, SPH_E_ARG, "x-slab sharding needs a single fluid density (uniform fluid masses)");
     if (halo_capacity < 1 || 2 * halo_capacity + ctx->P.n > ctx->n_max)
@@ -1152,6 +1174,19 @@ int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t 
     }
     ctx->shard_bodies = true;
     return SPH_OK;
+}
+}  // namespace
+extern "C" {
+
+int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                               int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
+    return shard_configure_bodies(ctx, false, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, bodies, n_bodies);
+}
+
+int sph_shard_configure_iisph_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers,
+                                     int64_t halo_capacity, int32_t rebalance_every, const SphRigidBody *bodies,
+                                     int32_t n_bodies) {
+    return shard_configure_bodies(ctx, true, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, bodies, n_bodies);
 }
 
 // the exchange at the end of sequence q delivers the records plan kernel q + 1 works on; that one re-balances
@@ -1437,8 +1472,8 @@ inline double *shard_err_parts(const SphCtx *c) { return reinterpret_cast<double
 // One exchange of the sharded DFSPH step with both neighbours: pack -> one transport group -> unpack.
 //   DX_ALIGN: the ghost alignment (4 record arrays of the sgw boundary layers + a 16-byte header per side), received
 //             into the receive regions behind the live records, which stay unused until the end-of-step exchange;
-//   DX_VELD / DX_DFS / DX_ACC / DX_AUX: one 16-byte word per particle of the outermost owned layer, received into the
-//             second staging array.
+//   DX_VELD / DX_DFS / DX_ACC / DX_AUX / DX_MISC: one 16-byte word per particle of the outermost owned layer, received
+//             into the second staging array.
 // Fixed-size messages (align_cap / sweep_cap records), so both sides always agree on the byte counts.  gather_err: the
 // same group also sends this rank's fp64 error partial (ctrl->err) to every other rank and receives theirs into
 // shard_err_parts() -- an all-gather of 8 bytes with plain send / recv.  ctrl (may be NULL): the pack and unpack of a
@@ -1566,6 +1601,9 @@ int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double et
 // constants in, counts out.  The exchanges run only on a sharded context: v* after predict_velocity (read by
 // k_iisph_predict), aux after k_iisph_predict (the warm-start p / rho^2 the first sweep reads), then the two of every
 // sweep.  compute_pressure_forces reads the aux words the converged sweep sent; nothing reads a ghost value after it.
+// Sharded with dynamic solids (c->shard_bodies): compute_pressure_forces runs without its reaction scatter (it would add
+// the reactions a second time, and onto ghost copies), the first ghost layer's final pressures arrive in one more
+// message (DX_MISC) and k_iisph_shard_reactions gathers the reactions onto the owned dynamic solids before the advect.
 int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n_grid, int64_t *kernels) {
     const DevParams &P = c->P;
     const int b128 = blocks_for(n_grid, 128), b256 = blocks_for(n_grid, 256);
@@ -1587,9 +1625,21 @@ int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n
                           kernels);
     if (rc) return rc;
     io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-    k_iisph_pressure_accel<true><<<b128, 128, 0, st>>>(P, c->S, nullptr);
+    if (c->shard_bodies) {
+        k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, c->S, nullptr);
+        *kernels += 1;
+        rc = shard_dfsph_exchange(c, st, DX_MISC, nullptr, false, kernels);
+        if (rc) return rc;
+        if (P.n_solid > 0) {
+            k_iisph_shard_reactions<<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S);
+            *kernels += 1;
+        }
+    } else {
+        k_iisph_pressure_accel<true><<<b128, 128, 0, st>>>(P, c->S, nullptr);
+        *kernels += 1;
+    }
     k_iisph_advect<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 2;
+    *kernels += 1;
     c->built = false; c->list_valid = false;  // positions moved
     return SPH_OK;
 }
@@ -1663,10 +1713,12 @@ int single_step(SphCtx *ctx, cudaStream_t st, Substep substep) {
     return SPH_OK;
 }
 
-// One sharded SPHBase.step() of a solver whose substep launches itself (DFSPH, IISPH; fluid + static solids; no
-// overlap of the exchanges with computation):
-//   plan -> classify + sort -> info -> DX ranges -> ghost alignment -> substep(n_grid) on owned records + ghosts
-//   -> clamp (owned) -> pack the send ranges -> the record exchange that feeds the next step's classification
+// One sharded SPHBase.step() of a solver whose substep launches itself (DFSPH, IISPH; no overlap of the exchanges with
+// computation):
+//   plan -> classify + sort -> info -> DX ranges -> ghost alignment [-> solid-id slot map -> moving boundary volumes]
+//   -> substep(n_grid) on owned records + ghosts [-> body all-gather + solve -> clamps of the other dynamic solids]
+//   -> clamp (owned fluid) -> pack the send ranges -> the record exchange that feeds the next step's classification
+// [..]: contexts with dynamic solids only (c->shard_bodies; IISPH, sph_shard_configure_iisph_bodies).
 template <typename Substep>
 int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels, Substep substep) {
     k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
@@ -1680,6 +1732,7 @@ int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels
     CUDA_TRY(c, cudaGetLastError());
     rc = shard_dfsph_exchange(c, st, DX_ALIGN, nullptr, false, kernels);
     if (rc) return rc;
+    if (c->shard_bodies) { rc = launch_shard_solid_slots(c, st, kernels); if (rc) return rc; }
     // The step waits on the host once per batch of sweeps anyway; one more short wait here for the live count lets
     // every substep launch cover [0, n_live) -- owned records and ghosts -- instead of the whole capacity.
     int32_t n_live = 0;
@@ -1688,7 +1741,8 @@ int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels
     const int64_t n_grid = std::min<int64_t>(std::max<int32_t>(n_live, 1), P.n);
     rc = substep(n_grid);
     if (rc) return rc;
-    // enforce_boundary_3D(fluid), sph_base.py:271 (no rigid solve before it: sharded contexts hold static solids only)
+    // solve_rigid_body(), enforce_boundary_3D(fluid) (sph_base.py:270-271)
+    if (c->shard_bodies) { rc = launch_shard_body_solve(c, st, kernels); if (rc) return rc; }
     k_enforce_boundary<<<blocks_for(n_grid, 256), 256, 0, st>>>(P, c->S, /*particle_type=*/1);
     // the advanced records of the send ranges -> staging, then the exchange the next step classifies
     k_shard_apply<<<dim3(blocks_for(P.halo_cap, 256), 2), 256, 0, st>>>(P, c->S, /*copy_all=*/1);
@@ -1842,7 +1896,6 @@ int sph_shard_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *st
     REQUIRE_SHARD(ctx);
     if (!io || nsteps < 0 || io->n_fluid < 1 || io->max_iterations < 1) return SPH_E_ARG;
     if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called before sph_shard_configure");
-    if (ctx->shard_bodies) return fail(ctx, SPH_E_ARG, kShardBodiesIisph);
     if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     if (ctx->world != ctx->shard_world)
         return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure: configure again");

@@ -329,11 +329,12 @@ enum {
     DX_INTS = 64
 };
 // what a pack / unpack moves: the alignment, or one 16-byte word per particle of one per-step array (DFSPH: veld, dfs;
-// IISPH: veld, acc = {a^p, fluid mark}, aux = {.., p / rho^2, ..})
-enum { DX_ALIGN = 0, DX_VELD = 1, DX_DFS = 2, DX_ACC = 3, DX_AUX = 4 };
+// IISPH: veld, acc = {a^p, fluid mark}, aux = {.., p / rho^2, ..}; IISPH with dynamic solids, once after the loop:
+// misc, of which only .y = the final pressure p lands on the ghost)
+enum { DX_ALIGN = 0, DX_VELD = 1, DX_DFS = 2, DX_ACC = 3, DX_AUX = 4, DX_MISC = 5 };
 
 __device__ __forceinline__ float4 *dx_sweep_array(const DevArrays &S, int what) {
-    return what == DX_VELD ? S.veld : what == DX_DFS ? S.dfs : what == DX_ACC ? S.acc : S.aux;
+    return what == DX_VELD ? S.veld : what == DX_DFS ? S.dfs : what == DX_ACC ? S.acc : what == DX_MISC ? S.misc : S.aux;
 }
 
 // After k_shard_info: the ranges above, and the alignment headers.  A range longer than its message capacity is cut
@@ -375,8 +376,8 @@ __global__ void k_dfsph_shard_ranges(DevParams P, DevArrays S, int32_t *dx, int 
 }
 
 // Pack what goes to the neighbours (blockIdx.y = side: 0 = to the left, 1 = to the right) into the send staging:
-// DX_ALIGN = the 4 records of the sgw boundary layers in this rank's sorted order, DX_VELD / DX_DFS / DX_ACC / DX_AUX =
-// one 16-byte word per particle of the outermost owned layer.  ctrl (may be NULL): a sweep behind the converged one has
+// DX_ALIGN = the 4 records of the sgw boundary layers in this rank's sorted order, DX_VELD / DX_DFS / DX_ACC / DX_AUX /
+// DX_MISC = one 16-byte word per particle of the outermost owned layer.  ctrl (may be NULL): a sweep behind the converged one has
 // nothing new.
 __global__ void k_dfsph_shard_pack(DevParams P, DevArrays S, const int32_t *dx, int what, const DfsphCtrl *ctrl) {
     if (ctrl && ctrl->done) return;
@@ -404,7 +405,8 @@ __global__ void k_dfsph_shard_pack(DevParams P, DevArrays S, const int32_t *dx, 
 // valid).  A count mismatch leaves the ghost range alone and a record of another cell is not written; both set
 // SPH_STATUS_GHOST_ALIGN.
 // DX_VELD / DX_DFS / DX_ACC / DX_AUX: rec[side][0] = the words of the neighbour's outermost owned layer -> this rank's
-// first ghost layer.
+// first ghost layer.  DX_MISC: only .y (the pressure) of each word -- misc.z carries FLAG_GHOST on this rank and not on
+// the owner, and the alignment already brought the rest.
 __global__ void k_dfsph_shard_unpack(DevParams P, DevArrays S, int32_t *dx, int what, const DfsphCtrl *ctrl,
                                      const float4 *rec00, const float4 *rec01, const float4 *rec02, const float4 *rec03,
                                      const float4 *rec10, const float4 *rec11, const float4 *rec12, const float4 *rec13) {
@@ -418,7 +420,8 @@ __global__ void k_dfsph_shard_unpack(DevParams P, DevArrays S, int32_t *dx, int 
     if (what != DX_ALIGN) {
         if (s >= e - b) return;
         SPH_EMU_CHECK(s < P.halo_cap && b + s >= 0 && b + s < P.n);
-        dx_sweep_array(S, what)[b + s] = r0[s];
+        if (what == DX_MISC) S.misc[b + s].y = r0[s].y;
+        else dx_sweep_array(S, what)[b + s] = r0[s];
         return;
     }
     const int32_t *h = dx + DX_HDR_RECV + 4 * side;

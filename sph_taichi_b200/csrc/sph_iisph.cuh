@@ -10,6 +10,9 @@
 // neighbours' values it reads in the first ghost layer -- v* in k_iisph_predict, aux.y = p / rho^2 in
 // k_iisph_pressure_accel, acc = {a^p, 1} in k_iisph_pressure_update -- arrive with the exchanges of the outermost owned
 // layer that the host issues after each kernel that changes them (DX_VELD, DX_AUX, DX_ACC).
+// Sharded with dynamic solids (sph_shard_configure_iisph_bodies): compute_pressure_forces runs without the reaction
+// scatter and k_iisph_shard_reactions gathers the same terms onto the owned dynamic solids, after one more exchange
+// (DX_MISC) that brings the first ghost layer's final pressures.
 //
 // Per-step scratch, all in existing per-step workspace (no new sorted payload):
 //   dfs[i]   = {a_ii, s_i, -, -}              (the DFSPH scratch; unused in an IISPH context)
@@ -103,6 +106,66 @@ __global__ void __launch_bounds__(128) k_iisph_pressure_accel(DevParams P, DevAr
         }
     });
     S.acc[i] = make_float4(P.rho0 * ax, P.rho0 * ay, P.rho0 * az, 1.0f);
+}
+
+// The reactions of compute_pressure_forces on the owned dynamic solids as a GATHER (sharded steps with dynamic solids;
+// the counterpart of k_shard_reactions): the scatter of k_iisph_pressure_accel<true> would miss the fluid a neighbour
+// owns across a cut.  One warp per solid id walks the 27 cells over the fluid records that hold this step's density
+// and final pressure -- the owned layers and the first ghost layer, [SD_DENS0, SD_DENS1) -- with the neighbour lists'
+// predicate (symmetric in i, b) and forms the solid branch of k_iisph_pressure_accel<true> operand for operand, so
+// only the summation order differs from the single engine's float atomics.  What it reads from a ghost fluid record i
+// and which message brought it: posm (alignment), veld.w = rho_i (DX_VELD, the owner's word), aux.y = p / rho^2 (the
+// converged sweep's DX_AUX; aux.z > 0 marks a fluid), misc.y = p (DX_MISC).  acc[b] holds {g, 0} from
+// k_dfsph_non_pressure; w stays 0.
+__global__ void __launch_bounds__(128) k_iisph_shard_reactions(DevParams P, DevArrays S) {
+    const int lane = threadIdx.x & 31;
+    const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (s >= P.n_solid) return;  // warp-uniform
+    const int b = S.solid_slot[s];
+    if (!shard_owned_index(S, b)) return;
+    if (!(__float_as_uint(S.misc[b].z) & FLAG_DYNAMIC)) return;
+    const float4 pb = S.posm[b];
+    const float rho_b = S.aux[b].x;  // the body density
+    const int d0 = S.sd[SD_DENS0], d1 = S.sd[SD_DENS1];
+    int ci, cj, ck;
+    cell_of(P, pb.x, pb.y, pb.z, ci, cj, ck);
+    ci = min(max(ci, 0), P.gx - 1); cj = min(max(cj, 0), P.gy - 1); ck = min(max(ck, 0), P.gz - 1);
+    const int k_lo = max(ck - 1, 0), k_hi = min(ck + 1, P.gz - 1);
+    float ax = 0.f, ay = 0.f, az = 0.f;
+    for (int dx = -1; dx <= 1; ++dx) {
+        int ni = ci + dx;
+        if (ni < 0 || ni >= P.gx) continue;
+        for (int dy = -1; dy <= 1; ++dy) {
+            int nj = cj + dy;
+            if (nj < 0 || nj >= P.gy) continue;
+            int row = (ni * P.gy + nj) * P.gz;
+            int i0 = max(__ldg(S.cell_end + max(row + k_lo - 1, 0)), d0);
+            int i1 = min(__ldg(S.cell_end + row + k_hi), d1);
+            for (int i = i0 + lane; i < i1; i += 32) {
+                const float4 ai = __ldg(S.aux + i);
+                if (!(ai.z > 0.0f)) continue;  // solid
+                const float4 pi = __ldg(S.posm + i);
+                float rx = pi.x - pb.x, ry = pi.y - pb.y, rz = pi.z - pb.z;
+                if (!(exact_r2(rx, ry, rz) < P.h2)) continue;  // the density pass's list predicate
+                const float gs = gradw_of(P, rx * rx + ry * ry + rz * rz);
+                const float c = pb.w * gs * (ai.y + __ldg(&S.misc[i].y) * P.inv_rho0sq);
+                const float f = -__ldg(&S.veld[i].w) / rho_b * P.rho0;
+                ax += -c * rx * f; ay += -c * ry * f; az += -c * rz * f;
+            }
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        ax += __shfl_xor_sync(0xffffffffu, ax, o);
+        ay += __shfl_xor_sync(0xffffffffu, ay, o);
+        az += __shfl_xor_sync(0xffffffffu, az, o);
+    }
+    if (lane != 0) return;
+    // the slot is read again rather than kept: with the divisions' slow-path calls in the loop, ptxas spilled it
+    float4 *ab = S.acc + S.solid_slot[(blockIdx.x * blockDim.x + threadIdx.x) >> 5];
+    float4 a = *ab;
+    a.x += ax; a.y += ay; a.z += az;
+    *ab = a;
 }
 
 // One sweep's second pass, with the sweep's error sum fused in (as k_dfsph_density_change_err):

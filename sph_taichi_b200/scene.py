@@ -187,6 +187,12 @@ def armadillo_bath_dynamic_dfsph():
     return _as_dfsph(armadillo_bath_dynamic())
 
 
+def armadillo_bath_dynamic_iisph():
+    """armadillo_bath_dynamic's geometry (three shape-matched armadillos) with the IISPH solver, dt = 1e-3: the
+    full-size scene of sharded IISPH with dynamic solids."""
+    return _as_iisph(armadillo_bath_dynamic())
+
+
 def box_4m_dfsph():
     """box_4m with the DFSPH solver (dt = 4e-3): the sharded DFSPH workload of bench.py --gpus N."""
     return _as_dfsph(box_4m())
@@ -201,6 +207,7 @@ NAMED_SCENES = {
     "dragon_bath_dynamic_dfsph": dragon_bath_dynamic_dfsph,
     "high_fluid_dfsph": high_fluid_dfsph,
     "armadillo_bath_dynamic_dfsph": armadillo_bath_dynamic_dfsph,
+    "armadillo_bath_dynamic_iisph": armadillo_bath_dynamic_iisph,
     "cube_8k": cube_8k,
     "box_4m": box_4m,
     "box_16m": box_16m,

@@ -39,8 +39,12 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
   the DFSPH step's shape with IISPH's substep: the once-per-step ghost alignment, the predicted velocities and the
   warm-start pressures of the outermost owned layer sent once per step, and two small exchanges per relaxed Jacobi
   sweep (its pressure accelerations, then its new pressures); the error sums are added in rank order, so every rank
-  runs the same sweeps (``last_iterations`` / ``last_avg_err``).  Fluid and static solids only: dynamic solids in
-  IISPH are refused (``DYNAMIC_SOLIDS_IISPH``).  Whether the sharded step beats one GPU at a given scene size depends
+  runs the same sweeps (``last_iterations`` / ``last_avg_err``).  Dynamic solids in IISPH are a second opt-in,
+  ``build_sharded(..., iisph_bodies=True)`` (``--gpus N --shard-iisph-bodies``, ``sph_shard_configure_iisph_bodies``);
+  with ``iisph=True`` alone they are refused (``DYNAMIC_SOLIDS_IISPH``).  IISPH scatters the reactions once per step,
+  after the pressure loop, so the WCSPH pieces carry over: 3 ghost layers with moving boundary volumes, the final
+  pressure acceleration without the scatter, one more message with the first ghost layer's final pressures, the
+  reactions gathered onto the owned dynamic solids, and the bodies solved on every rank from the all-gather.  Whether the sharded step beats one GPU at a given scene size depends
   on the sweep count: each sweep costs two transport groups and each batch of sweeps one host wait.
 * Output: ``ShardedSimulation.dump(obj_id)`` is ``ParticleSystem.dump`` of a sharded run.  It is collective: every rank
   compacts x and v of that object's owned records on the device and rank 0 receives them over the engine's own
@@ -82,7 +86,8 @@ IISPH_SINGLE_GPU = ("IISPH (simulationMethod 3) is single-GPU unless sharding is
 DYNAMIC_SOLIDS_WCSPH_ONLY = ("x-slab sharding of dynamic solids is WCSPH only: the DFSPH pressure sweeps scatter the "
                              "reactions onto the bodies in every sweep, which would need a reaction exchange per sweep")
 DYNAMIC_SOLIDS_IISPH = ("x-slab sharding of dynamic solids is WCSPH only: dynamic solids in IISPH scenes are single-GPU "
-                        "(sharded IISPH runs fluid and static solids)")
+                        "unless requested: build_sharded(..., iisph_bodies=True) / run_simulation.py --gpus N "
+                        "--shard-iisph-bodies (sharded IISPH otherwise runs fluid and static solids)")
 
 
 def scene_params(cfg):
@@ -266,12 +271,13 @@ class ShardedSimulation:
     """This rank's share of a sharded scene: a CUDA engine in slab mode + the library's halo exchange."""
 
     def __init__(self, cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, uniform_hint, group=None,
-                 rebalance_every=8, transport=None, n_fluid=None, n_solid=0, bodies=None):
+                 rebalance_every=8, transport=None, n_fluid=None, n_solid=0, bodies=None, iisph_bodies=False):
         """``mine``: this rank's initial particles (numpy arrays in the reference's field layout); with solids also
         ``solid_id`` (global ids, ``solid_ids``) and ``m_V`` (start-up boundary volumes, ``startup_boundary_volumes``).
-        ``n_solid``: the solid count of the WHOLE scene (sizes the solid-id slot map).  ``bodies`` (dynamic solids,
-        WCSPH): [(object_id, solid_begin, solid_end, rest_cm)] of the whole scene (``dynamic_bodies``,
-        ``startup_rest_cms``), an empty list for advected rigid blocks only; None refuses dynamic solids."""
+        ``n_solid``: the solid count of the WHOLE scene (sizes the solid-id slot map).  ``bodies`` (dynamic solids;
+        WCSPH, or IISPH with ``iisph_bodies=True``): [(object_id, solid_begin, solid_end, rest_cm)] of the whole scene
+        (``dynamic_bodies``, ``startup_rest_cms``), an empty list for advected rigid blocks only; None refuses dynamic
+        solids."""
         from . import engine as _engine
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dfsph = cfg.get_cfg("simulationMethod") == 4
@@ -289,7 +295,7 @@ class ShardedSimulation:
         self.bodies = None if bodies is None else list(bodies)
         if self.bodies is not None and self.dfsph:
             raise NotImplementedError(DYNAMIC_SOLIDS_WCSPH_ONLY)
-        if self.bodies is not None and self.iisph:
+        if self.bodies is not None and self.iisph and not iisph_bodies:
             raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
         self.eng = _engine.Engine(scene_params(cfg), n_max=self.n_cap, n_solid=self.n_solid,
                                   n_bodies=len(self.bodies or []), device=self.device)
@@ -331,9 +337,9 @@ class ShardedSimulation:
             for i, (oid, b0, b1, rest_cm) in enumerate(self.bodies):
                 table[i].object_id, table[i].solid_begin, table[i].solid_end = int(oid), int(b0), int(b1)
                 table[i].rest_cm = (C.c_float * 3)(*[float(v) for v in rest_cm])
-            e._check(e.lib.sph_shard_configure_bodies(e.ctx, lo, hi, GHOST_LAYERS_BODIES, self.halo_cap,
-                                                      int(rebalance_every), table, len(self.bodies)),
-                     "sph_shard_configure_bodies")
+            name = "sph_shard_configure_iisph_bodies" if self.iisph else "sph_shard_configure_bodies"
+            e._check(getattr(e.lib, name)(e.ctx, lo, hi, GHOST_LAYERS_BODIES, self.halo_cap, int(rebalance_every),
+                                          table, len(self.bodies)), name)
         e._check(e.lib.sph_shard_begin(e.ctx, e._stream()), "sph_shard_begin")
         self.steps_done = 0
         # the scene's objects and per-object particle counts (build_sharded sets them; dump() sizes rank 0's buffers
@@ -499,25 +505,31 @@ class ShardedSimulation:
 
 
 def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1.2, rebalance_every=8, slabs=None,
-                  transport=None, dynamic_solids=False, iisph=False):
+                  transport=None, dynamic_solids=False, iisph=False, iisph_bodies=False):
     """Assemble the scene on every rank, plan the slabs from the initial layer histogram and load this rank's
     share into a CUDA engine.  ``dynamic_solids=True`` opts in to sharding WCSPH scenes with dynamic solids
     (3 ghost layers, reactions gathered across cuts, bodies solved on every rank from an all-gather of their particles).
-    ``iisph=True`` opts in to sharding an IISPH scene (fluid and static solids).
+    ``iisph=True`` opts in to sharding an IISPH scene (fluid and static solids); ``iisph_bodies=True`` to sharding an
+    IISPH scene with dynamic solids (it implies ``iisph`` and the layout of ``dynamic_solids``).
     Returns (ShardedSimulation, n_total)."""
     from .config_builder import SimConfig
     from .scene import assemble_particles
 
     cfg = SimConfig(scene_dict)
     method = cfg.get_cfg("simulationMethod")
-    if method == 3 and not iisph:
+    if iisph_bodies and method != 3:
+        raise ValueError(f"iisph_bodies=True shards an IISPH scene (simulationMethod 3) with dynamic solids, not "
+                         f"simulationMethod {method}")
+    if method == 3 and not (iisph or iisph_bodies):
         raise NotImplementedError(IISPH_SINGLE_GPU)
     if method not in (0, 3, 4):
         raise NotImplementedError(f"x-slab sharding runs WCSPH (0), DFSPH (4) and IISPH (3) scenes, not "
                                   f"simulationMethod {method}")
     if iisph and method != 3:
         raise ValueError(f"iisph=True shards an IISPH scene (simulationMethod 3), not simulationMethod {method}")
-    if iisph and (dynamic_solids or any(o.get("isDynamic") for o in
+    if iisph_bodies:
+        iisph = dynamic_solids = True
+    elif iisph and (dynamic_solids or any(o.get("isDynamic") for o in
                                         list(cfg.get_rigid_bodies() or []) + list(cfg.get_rigid_blocks() or []))):
         raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
     radius = cfg.get_cfg("particleRadius")
@@ -559,7 +571,7 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     n_cap = int((n_mine + ghost_est) * capacity_factor) + 4 * halo_cap + 1024  # live + trash + 2 receive regions
     sim = ShardedSimulation(cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, hint, group=group,
                             rebalance_every=rebalance_every, transport=transport, n_fluid=int(fluid.sum()),
-                            n_solid=n_solid, bodies=bodies)
+                            n_solid=n_solid, bodies=bodies, iisph_bodies=iisph_bodies)
     sim.object_collection = object_collection  # the meshes of the OBJ export (restPosition, restCenterOfMass)
     sim.object_counts = {int(o): int(k) for o, k in zip(object_ids, object_sizes)}
     return sim, counts["total"]

@@ -28,7 +28,11 @@ a few steps, so the pressure solves of DFSPH and IISPH run several sweeps right 
 start -- and resting on the fluid surface, and an advected dynamic rigid block on the surface at 3/4 of the fluid.  The tool then also reports whether
 every body's cm and R were bit-identical on every rank after every step, whether the fluid's reactions acted (every
 dynamic object's mean velocity left free fall, in both engines), and the per-body cm / R differences; "ok" then also
-requires max_dv < 1e-2 and per-body |dcm| / d and max |dR| below 1e-3.
+requires max_dv < 1e-2 and per-body |dcm| / d and max |dR| below 1e-3.  --body-vy gives the dynamic solids an initial
+vertical velocity (a body thrown into the fluid raises pressures under it within a few steps).
+
+--iisph together with --dynamic-body / --dynamic-block builds with build_sharded(iisph_bodies=True) and reports both
+sets: the sweep counts, their equality across ranks and the ghost alignment, and the body and reaction checks.
 """
 import argparse
 import json
@@ -75,8 +79,9 @@ def colliding_blocks_scene(c, d, vx):
     return sc
 
 
-def add_dynamic_solids(sc, c, d, world, body, block):
-    """The dynamic solids of --dynamic-body / --dynamic-block on top of the dam break of ``c`` particles (start 0.06)."""
+def add_dynamic_solids(sc, c, d, world, body, block, vy=0.0):
+    """The dynamic solids of --dynamic-body / --dynamic-block on top of the dam break of ``c`` particles (start 0.06),
+    with the initial vertical velocity ``vy``."""
     x0, top, z0 = 0.06, 0.06 + c[1] * d, 0.06
     side = 4.5 * d
     if body:
@@ -84,25 +89,25 @@ def add_dynamic_solids(sc, c, d, world, body, block):
         sc.setdefault("RigidBodies", []).append({
             "objectId": 2, "geometryFile": os.path.join(ROOT, "tests", "golden", "cube.obj"),
             "translation": [cut - side / 2, top + 0.25 * d, z0 + (c[2] * d - side) / 2], "rotationAxis": [0, 1, 0],
-            "rotationAngle": 0, "scale": [side] * 3, "velocity": [0.0, 0.0, 0.0], "density": 800.0,
+            "rotationAngle": 0, "scale": [side] * 3, "velocity": [0.0, vy, 0.0], "density": 800.0,
             "color": [255, 255, 255], "isDynamic": True})
     if block:
         bx = x0 + 0.75 * c[0] * d
         sc.setdefault("RigidBlocks", []).append({
             "objectId": 3, "start": [bx, top, z0 + d], "end": [bx + 2.5 * d, top + 2.5 * d, z0 + 3.5 * d],
-            "translation": [0.0, 0.0, 0.0], "scale": [1, 1, 1], "velocity": [0.0, 0.0, 0.0], "density": 600.0,
+            "translation": [0.0, 0.0, 0.0], "scale": [1, 1, 1], "velocity": [0.0, vy, 0.0], "density": 600.0,
             "color": [255, 0, 0], "isDynamic": True})
     return sc
 
 
-def dynamic_velocities(V, OID, FL, g_y, t):
-    """{object_id: (mean v_y, deviation from free fall)} of the dynamic solids (objects start at rest)."""
+def dynamic_velocities(V, OID, FL, g_y, t, vy0=0.0):
+    """{object_id: (mean v_y, deviation from free fall)} of the dynamic solids (objects start at v_y = ``vy0``)."""
     out = {}
     dyn = (FL & 3) == 2
     for oid in sorted(set(OID[dyn].tolist())):
         m = dyn & (OID == oid)
         vy = float(V[m][:, 1].double().mean())
-        out[int(oid)] = (vy, abs(vy - g_y * t))
+        out[int(oid)] = (vy, abs(vy - vy0 - g_y * t))
     return out
 
 
@@ -120,8 +125,11 @@ def main():
                     help="the fluid rests on a static rigid block that straddles every cut (static_block_scene)")
     ap.add_argument("--collide", action="store_true",
                     help="two fluid blocks meeting at +-vx at the initial cut (colliding_blocks_scene)")
-    ap.add_argument("--dynamic-body", action="store_true", help="a shape-matched cube across the initial cut (WCSPH)")
-    ap.add_argument("--dynamic-block", action="store_true", help="an advected dynamic rigid block (WCSPH)")
+    ap.add_argument("--dynamic-body", action="store_true",
+                    help="a shape-matched cube across the initial cut (WCSPH; with --iisph: iisph_bodies=True)")
+    ap.add_argument("--dynamic-block", action="store_true",
+                    help="an advected dynamic rigid block (WCSPH; with --iisph: iisph_bodies=True)")
+    ap.add_argument("--body-vy", type=float, default=0.0, help="initial vertical velocity of the dynamic solids")
     ap.add_argument("--scene", default=None, choices=sorted(scene.NAMED_SCENES),
                     help="a named scene as it is (--counts, --vx and --static-block do not apply; a DFSPH scene needs "
                          "--dfsph for the iteration-count comparison, an IISPH scene --iisph)")
@@ -152,7 +160,7 @@ def main():
         sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12], start=[0.06] * 3)
     dynamic = a.dynamic_body or a.dynamic_block
     if dynamic and not a.scene:
-        sc = add_dynamic_solids(sc, c, d, world, a.dynamic_body, a.dynamic_block)
+        sc = add_dynamic_solids(sc, c, d, world, a.dynamic_body, a.dynamic_block, a.body_vy)
     if a.scene and any(b.get("isDynamic") for b in sc.get("RigidBodies", []) + sc.get("RigidBlocks", [])):
         dynamic = True
     if not a.scene and not a.collide:
@@ -175,9 +183,15 @@ def main():
         cuts = [cuts[0]] + [c_ + a.skew for c_ in cuts[1:-1]] + [cuts[-1]]
         slabs = [(cuts[r], cuts[r + 1]) for r in range(world)]
     sim, n_total = slab.build_sharded(sc, rank, world, dev, rebalance_every=a.rebalance_every, slabs=slabs,
-                                      transport=transport, dynamic_solids=dynamic, iisph=a.iisph)
+                                      transport=transport, dynamic_solids=dynamic, iisph=a.iisph,
+                                      iisph_bodies=bool(a.iisph and dynamic))
     first = sim.info()
     trace = []
+
+    def body_trace():
+        return [[c_.tobytes().hex(), R_.tobytes().hex()] for c_, R_ in
+                (sim.body_state(b) for b in range(len(sim.bodies)))]
+
     if a.soak:
         done = 0
         while done < a.steps:
@@ -193,18 +207,17 @@ def main():
     elif a.iisph:
         for _ in range(a.steps):  # one step per call: the sweep counts of every step
             sim.step(1)
-            trace.append((sim.last_iterations, sim.last_avg_err.hex()))
+            trace.append((sim.last_iterations, sim.last_avg_err.hex()) + ((body_trace(),) if dynamic else ()))
     elif dynamic:
         for _ in range(a.steps):  # one step per call: the body states of every step
             sim.step(1)
-            trace.append([[c_.tobytes().hex(), R_.tobytes().hex()] for c_, R_ in
-                          (sim.body_state(b) for b in range(len(sim.bodies)))])
+            trace.append(body_trace())
     else:
         sim.step(a.steps)
     last = sim.info()
     gathered = slab.gather_owned(sim)
     meta = {"owned": (first["owned"], last["owned"]), "halo": 64 * last["halo_records_sent"], "trace": trace,
-            "slab0": (first["x_lo"], first["x_hi"]), "slab1": (last["x_lo"], last["x_hi"])}
+            "slab0": (first["x_lo"], first["x_hi"]), "slab1": (last["x_lo"], last["x_hi"]), "status": last["status"]}
     if jacobi:
         # the x_0 of the ghost layers ([0, own_begin) and [own_end, n_live)) and of the owned records, as the last
         # step's alignment left them (advect and clamp touch owned records only; the sort comes with the next step)
@@ -278,21 +291,22 @@ def main():
             if a.iisph:
                 cmp_.update(avg_err_sharded=[float.fromhex(t[1]) for t in metas[0]["trace"]], avg_err_single=single_errs)
         if dynamic:
-            same_on_ranks = all(m["trace"] == metas[0]["trace"] for m in metas)
+            same_on_ranks = all(json.dumps(m["trace"]) == json.dumps(metas[0]["trace"]) for m in metas)
             g_y, t = float(sc["Configuration"]["gravitation"][1]), a.steps * float(sc["Configuration"]["timeStepSize"])
             X, V, X0, OID, MV, FL = gathered
-            vs = dynamic_velocities(V, OID, FL, g_y, t)
+            vs = dynamic_velocities(V, OID, FL, g_y, t, a.body_vy)
             ps._pull()
             n_ = int(ps.particle_num[None])
             fl1 = (ps._t["material"][:n_] != 1).int() * 2 * (ps._t["is_dynamic"][:n_] != 0).int()
-            v1 = dynamic_velocities(ps._t["v"][:n_], ps._t["object_id"][:n_], fl1, g_y, t)
+            v1 = dynamic_velocities(ps._t["v"][:n_], ps._t["object_id"][:n_], fl1, g_y, t, a.body_vy)
             acted = bool(vs) and all(vs[o][1] > 1e-3 and v1[o][1] > 1e-3 for o in vs)
             bodies_ok = all(b["dcm_over_d"] < 1e-3 and b["max_dR"] < 1e-3 for b in cmp_.get("bodies", []))
             ok = (cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < 1e-3 and cmp_["max_dv"] < 1e-2
-                  and same_on_ranks and bodies_ok and slab.static_solids_ok(cmp_))
+                  and same_on_ranks and bodies_ok and slab.static_solids_ok(cmp_)
+                  and (not jacobi or cmp_["ghosts_aligned"]))
             cmp_ = dict(cmp_, bodies_bit_identical_across_ranks=same_on_ranks, reactions_acted=acted,
                         dynamic_vy_sharded={str(k): v[0] for k, v in vs.items()},
-                        dynamic_vy_single={str(k): v[0] for k, v in v1.items()}, free_fall_vy=g_y * t,
+                        dynamic_vy_single={str(k): v[0] for k, v in v1.items()}, free_fall_vy=a.body_vy + g_y * t,
                         n_bodies=len(sim.bodies), transport_groups=[m["transport"][0] for m in metas],
                         transport_bytes=[m["transport"][1] for m in metas], halo_cap=[m["halo_cap"] for m in metas],
                         body_particles=metas[0]["body_particles"])
@@ -314,7 +328,8 @@ def main():
         print(json.dumps(dict(cmp_, world=world, particles=int(n_total), steps=a.steps, migrated=bool(migrated),
                               cuts_moved=bool(moved), owned_first_last=[list(map(int, m["owned"])) for m in metas],
                               slabs_first=[list(m["slab0"]) for m in metas], slabs_last=[list(m["slab1"]) for m in metas],
-                              halo_bytes=[int(m["halo"]) for m in metas], ok=bool(ok))))
+                              halo_bytes=[int(m["halo"]) for m in metas], status=[int(m["status"]) for m in metas],
+                              ok=bool(ok))))
     if world > 1:
         flag = torch.tensor([1 if ok else 0], device=dev)
         dist.broadcast(flag, src=0)

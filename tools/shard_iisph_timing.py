@@ -8,7 +8,12 @@ of the live count and the rank-ordered loop check to the plain one; at world 1 i
 nothing.  The card's name and power limit are read in the same run.  Writes one JSON object to `--out` (default
 profiles/h100_shard_iisph_timing.json) and prints a summary line.
 
-    python tools/shard_iisph_timing.py [--steps 20] [--rounds 5] [--warmup 30] [--out PATH]
+`--bodies` times sharded IISPH with dynamic solids instead (scene armadillo_bath_dynamic_iisph, built with
+`build_sharded(iisph_bodies=True)`; default output profiles/h100_shard_iisph_bodies_timing.json): the sharded step then
+also rebuilds the solid-id slot map, computes the moving boundary volumes through it, gathers the reactions instead of
+scattering them and solves the bodies from the packed table of their particles.
+
+    python tools/shard_iisph_timing.py [--bodies] [--steps 20] [--rounds 5] [--warmup 30] [--out PATH]
 """
 import argparse
 import json
@@ -38,18 +43,23 @@ def timed(step, last_sweeps, k):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--scene", default="dragon_bath_iisph")
+    ap.add_argument("--scene", default=None, help="default: dragon_bath_iisph, with --bodies "
+                                                  "armadillo_bath_dynamic_iisph")
+    ap.add_argument("--bodies", action="store_true", help="a scene with dynamic solids: build_sharded(iisph_bodies=True)")
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=30)
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_shard_iisph_timing.json"))
+    ap.add_argument("--out", default=None)
     a = ap.parse_args()
+    a.scene = a.scene or ("armadillo_bath_dynamic_iisph" if a.bodies else "dragon_bath_iisph")
+    a.out = a.out or os.path.join(ROOT, "profiles", "h100_shard_iisph_bodies_timing.json" if a.bodies
+                                  else "h100_shard_iisph_timing.json")
     dev = torch.device("cuda:0")
     sc = scene.NAMED_SCENES[a.scene]()
     ps = ParticleSystem(SimConfig(sc), device=dev)
     solver = ps.build_solver()
     solver.initialize()
-    sim, n_total = slab.build_sharded(scene.NAMED_SCENES[a.scene](), 0, 1, dev, iisph=True)
+    sim, n_total = slab.build_sharded(scene.NAMED_SCENES[a.scene](), 0, 1, dev, iisph=True, iisph_bodies=a.bodies)
     engines = {"plain": (lambda: solver.step(1), lambda: int(solver.last_iterations)),
                "sharded_world1": (lambda: sim.step(1), lambda: int(sim.last_iterations))}
     for step, _ in engines.values():
