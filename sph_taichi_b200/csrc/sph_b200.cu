@@ -46,6 +46,13 @@ const char *const kShardIisphBodiesContext =
     "(WCSPH contexts use sph_shard_configure_bodies; dynamic solids in DFSPH are single-GPU)";
 const char *const kShardBodiesFixed =
     "the body table of a context configured by sph_shard_configure_bodies is fixed: configure a new context";
+const char *const kNoDfsph = "sph_set_dfsph(1) was not called";
+const char *const kNoIisph = "sph_set_iisph(1) was not called";
+const char *const kWorldChanged = "the transport's world size changed after sph_shard_configure: configure again";
+// device copy P.dfsph, set for IISPH too: the two Jacobi solvers share the density pass (no clamp, no EOS)
+enum class Solver { WCSPH, DFSPH, IISPH };
+// device copy P.slab_on; Static: sph_shard_configure, Bodies: sph_shard_configure_bodies / _iisph_bodies
+enum class ShardMode { Off, Static, Bodies };
 
 constexpr int NUM_TIMERS = 12;
 constexpr int GRAPH_UNROLL = 4;  // must be even (ping-pong parity returns to its start)
@@ -191,7 +198,7 @@ struct SphCtx {
     cudaStream_t capture_stream = nullptr;  // graphs are captured here (the legacy stream cannot capture)
     bool built = false;  // neighbour structure valid for current positions
     bool list_valid = false;  // neighbour lists valid for current positions (DFSPH kernels)
-    bool iisph = false;  // sph_set_iisph(1): P.dfsph is set too (the density pass of both is the same)
+    Solver solver = Solver::WCSPH;  // written by set_solver only, together with P.dfsph
     // x-slab sharding (sph_shard_*)
     SphTransport transport{};
     bool has_transport = false;
@@ -211,10 +218,9 @@ struct SphCtx {
     int64_t shard_sequences = 0;  // sequences run so far (begin = 0): sequence q feeds the plan kernel of q + 1
     // sharded DFSPH: records per side of the ghost alignment (sgw layers) and of a per-sweep exchange (one layer)
     int32_t align_cap = 0, sweep_cap = 0;
-    int shard_world = 1;  // world size the shard buffer's per-rank error partials were sized for
-    // configured by sph_shard_configure_bodies (WCSPH: steps with shard_bodies_sequence) or
-    // sph_shard_configure_iisph_bodies (IISPH: shard_dfsph_sequence with its body hooks)
-    bool shard_bodies = false;
+    int shard_world = 1;  // world size the shard buffer's per-rank error partials and body tables were sized for
+    // Bodies: a WCSPH context steps with shard_bodies_sequence, an IISPH one with shard_dfsph_sequence's body hooks
+    ShardMode shard = ShardMode::Off;  // set by shard_setup and shard_configure_bodies, together with P.slab_on
     uint64_t xfer_groups = 0, xfer_bytes = 0;  // transport groups issued from the host, and the bytes this rank sent
     // sph_shard_dump's device scratch (library-owned, grown on demand): the header sent, the headers received, the
     // tile counts
@@ -227,6 +233,43 @@ namespace {
 int fail(SphCtx *ctx, int code, const std::string &msg) {
     if (ctx) ctx->err = msg; else g_create_error = msg;
     return code;
+}
+
+// What an entry point needs of a context's solver and shard mode.  A NULL refusal message means no such requirement;
+// the messages that differ between entry points are the entry point's own.
+struct Need {
+    bool configured = false, begun = false, grid = false, lists = false;
+    Solver solver = Solver::WCSPH;
+    const char *other_solver = nullptr, *if_sharded = nullptr, *if_bodies = nullptr, *if_moved = nullptr;
+    Need &sharded() { configured = true; return *this; }
+    Need &runs(Solver s, const char *refusal) { solver = s; other_solver = refusal; return *this; }
+    Need &shard_step(Solver s, const char *refusal) { configured = begun = true; return runs(s, refusal); }
+    Need &unsharded(const char *refusal) { if_sharded = refusal; return *this; }
+    Need &no_bodies(const char *refusal) { if_bodies = refusal; return *this; }
+    Need &same_world(const char *refusal) { if_moved = refusal; return *this; }
+    Need &built() { grid = true; return *this; }  // neighbour structure valid, unless there are no particles
+    Need &fresh_lists() { lists = true; return *this; }  // neighbour lists valid too
+};
+
+// The mode checks of every entry point, in this order: configured, the entry point's bare argument checks (args_ok),
+// solver, not sharded, not a body context, begun, world size unchanged, then the neighbour structure; returns the first
+// refusal or SPH_OK.  Other solvers' entry points refuse an IISPH context with one message per kind (sharded or not).
+int require(SphCtx *c, const Need &n, bool args_ok = true) {
+    if (!c) return SPH_E_ARG;
+    if (n.configured && c->shard == ShardMode::Off) return fail(c, SPH_E_ARG, "sph_shard_configure was not called");
+    if (!args_ok) return SPH_E_ARG;
+    if (n.other_solver && c->solver != n.solver)
+        return fail(c, SPH_E_ARG, c->solver == Solver::IISPH ? (n.configured ? kIisphShardStep : kIisphContext) : n.other_solver);
+    if (n.if_sharded && c->shard != ShardMode::Off) return fail(c, SPH_E_ARG, n.if_sharded);
+    if (n.if_bodies && c->shard == ShardMode::Bodies) return fail(c, SPH_E_ARG, n.if_bodies);
+    if (n.begun && !c->shard_begun) return fail(c, SPH_E_ARG, "sph_shard_begin was not called");
+    if (n.if_moved && c->world != c->shard_world) return fail(c, SPH_E_ARG, n.if_moved);
+    if (n.grid && c->P.n > 0 && !c->built)
+        return fail(c, SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first (the reference's kernels "
+                                  "would read an outdated grid here)");
+    if (n.lists && (!c->built || !c->list_valid))
+        return fail(c, SPH_E_ARG, "neighbour lists are stale: run sph_neighbor_build and op 0 (compute_densities) first");
+    return SPH_OK;
 }
 
 #define CUDA_TRY(ctx, expr)                                                                        \
@@ -286,8 +329,6 @@ void bind_arrays(SphCtx *c) {
 
 inline RigidBodyDev *dev_bodies(SphCtx *c) { return reinterpret_cast<RigidBodyDev *>(c->ws + c->L.off_bodies); }
 int store_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodies);
-int shard_setup(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
-                int32_t rebalance_every, int64_t n_body_particles);
 
 inline int blocks_for(int64_t n, int t) { return (int)((n + t - 1) / t); }
 // Sharded steps: n is the capacity and the real counts are device state, so the LIGHT step kernels (histogram,
@@ -326,6 +367,8 @@ void drop_graphs(SphCtx *c) {
         for (int w = 0; w < 2; ++w) drop(c->graph_shard[k][w]);
     }
 }
+
+void set_solver(SphCtx *c, Solver s) { c->solver = s; c->P.dfsph = s != Solver::WCSPH; drop_graphs(c); }
 
 // ---- launch sequences -----------------------------------------------------------------
 struct StageTimer {
@@ -580,7 +623,7 @@ int sph_pack(SphCtx *ctx, const SphFields *f, int64_t n, void *stream) {
 int sph_set_solid_count(SphCtx *ctx, int64_t n_solid, int32_t has_dynamic_solids) {
     if (!ctx) return SPH_E_ARG;
     if (n_solid < 0 || n_solid > ctx->n_solid_cap) return fail(ctx, SPH_E_CAPACITY, "n_solid exceeds the capacity given at creation");
-    if (ctx->P.slab_on && n_solid > 0 && has_dynamic_solids) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
+    if (int rc = require(ctx, Need().unsharded(n_solid > 0 && has_dynamic_solids ? kShardStaticOnly : nullptr))) return rc;
     ctx->P.n_solid = (int32_t)n_solid;
     ctx->has_dynamic_solids = has_dynamic_solids != 0;
     drop_graphs(ctx);
@@ -636,21 +679,15 @@ int sph_neighbor_build(SphCtx *ctx, void *stream) {
     return launch_neighbor_build(ctx, static_cast<cudaStream_t>(stream), nullptr, &ctx->launches);
 }
 
-#define REQUIRE_BUILT(ctx)                                                                                  \
-    if (!(ctx)) return SPH_E_ARG;                                                                           \
-    if ((ctx)->P.n == 0) return SPH_OK;                                                                     \
-    if (!(ctx)->built)                                                                                      \
-        return fail((ctx), SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first "        \
-                                      "(the reference's kernels would read an outdated grid here)");
-
 int sph_boundary_volume(SphCtx *ctx, int32_t moving, void *stream) {
-    if (ctx && ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
-    REQUIRE_BUILT(ctx);
+    if (int rc = require(ctx, Need().unsharded(kShardStaticOnly).built())) return rc;
+    if (ctx->P.n == 0) return SPH_OK;
     return launch_boundary_volume(ctx, moving, static_cast<cudaStream_t>(stream), &ctx->launches);
 }
 
 int sph_compute_densities(SphCtx *ctx, void *stream) {
-    REQUIRE_BUILT(ctx);
+    if (int rc = require(ctx, Need().built())) return rc;
+    if (ctx->P.n == 0) return SPH_OK;
     k_density_simple<<<blocks_for(ctx->P.n, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S);
     ctx->launches += 1;
     CUDA_TRY(ctx, cudaGetLastError());
@@ -658,7 +695,8 @@ int sph_compute_densities(SphCtx *ctx, void *stream) {
 }
 
 int sph_compute_non_pressure_forces(SphCtx *ctx, void *stream) {
-    REQUIRE_BUILT(ctx);
+    if (int rc = require(ctx, Need().built())) return rc;
+    if (ctx->P.n == 0) return SPH_OK;
     k_force_simple<true, false><<<blocks_for(ctx->P.n, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S);
     ctx->launches += 1;
     CUDA_TRY(ctx, cudaGetLastError());
@@ -666,7 +704,8 @@ int sph_compute_non_pressure_forces(SphCtx *ctx, void *stream) {
 }
 
 int sph_compute_pressure_forces(SphCtx *ctx, void *stream) {
-    REQUIRE_BUILT(ctx);
+    if (int rc = require(ctx, Need().built())) return rc;
+    if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     k_eos<<<blocks_for(ctx->P.n, 256), 256, 0, st>>>(ctx->P, ctx->S);
     k_force_simple<false, true><<<blocks_for(ctx->P.n, 128), 128, 0, st>>>(ctx->P, ctx->S);
@@ -698,8 +737,7 @@ int sph_enforce_boundary(SphCtx *ctx, int32_t particle_type, void *stream) {
 int sph_set_rigid_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodies) {
     if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
     if (n_bodies > ctx->body_cap) return fail(ctx, SPH_E_CAPACITY, "more rigid bodies than the workspace was sized for");
-    if (ctx->P.slab_on && n_bodies > 0) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
-    if (ctx->shard_bodies) return fail(ctx, SPH_E_ARG, kShardBodiesFixed);
+    if (int rc = require(ctx, Need().unsharded(n_bodies > 0 ? kShardStaticOnly : nullptr).no_bodies(kShardBodiesFixed))) return rc;
     for (int b = 0; b < n_bodies; ++b)  // validate everything before any state changes
         if (bodies[b].solid_begin < 0 || bodies[b].solid_end < bodies[b].solid_begin || bodies[b].solid_end > ctx->n_solid_cap)
             return fail(ctx, SPH_E_ARG, "rigid body solid-id range out of bounds");
@@ -728,8 +766,7 @@ int store_bodies(SphCtx *ctx, const SphRigidBody *bodies, int32_t n_bodies) {
 extern "C" {
 
 static int rigid_call(SphCtx *ctx, int32_t body, int mode, float *out, void *stream) {
-    if (!ctx) return SPH_E_ARG;
-    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kShardStaticOnly);
+    if (int rc = require(ctx, Need().unsharded(kShardStaticOnly))) return rc;
     if (body < 0 || body >= (int)ctx->bodies.size()) return fail(ctx, SPH_E_ARG, "rigid body index out of range");
     k_rigid<<<1, RIGID_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S, dev_bodies(ctx), body, mode, out, 0);
     ctx->launches += 1;
@@ -757,9 +794,8 @@ int sph_get_rigid_state(SphCtx *ctx, int32_t body, float *out_dev12, void *strea
 }
 
 int sph_step(SphCtx *ctx, int32_t nsteps, void *stream) {
-    if (!ctx || nsteps < 0) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
-    if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_step is the fused WCSPH step; DFSPH is driven through sph_dfsph_op");
+    const char *dfsph = "sph_step is the fused WCSPH step; DFSPH is driven through sph_dfsph_op";
+    if (int rc = require(ctx, Need().runs(Solver::WCSPH, dfsph), nsteps >= 0)) return rc;
     if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int s = 0;
@@ -877,19 +913,26 @@ int shard_exchange(SphCtx *c, cudaStream_t st, bool wide) {
         [] { return SPH_OK; });
 }
 
-// plan -> classify + sort -> info -> boundary densities -> boundary forces (-> staging) ->
-// { exchange || interior densities -> apply -> interior forces }
-// ev[8] (optional): CUDA events at the stage boundaries, [5..6] around the exchange, [7] after the interior
-// densities (sph_shard_profile_step)
+// The opening of every sharded sequence: plan -> classify + sort -> info.
 // wide: this sequence's exchange feeds a re-balancing step and carries sgw + 2 layers instead of sgw + 1
-int shard_sequence(SphCtx *c, cudaStream_t st, bool compute, bool wide, int64_t *kernels, cudaEvent_t *ev = nullptr) {
-    if (ev) cudaEventRecord(ev[0], st);
+int shard_sort(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels) {
     k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
     *kernels += 1;
     int rc = launch_neighbor_build(c, st, nullptr, kernels, /*move_acc=*/false);
     if (rc) return rc;
     k_shard_info<<<1, 32, 0, st>>>(c->P, c->S, c->P.sgw + (wide ? 2 : 1), wide ? c->P.halo_cap : c->narrow_cap);
     *kernels += 1;
+    return SPH_OK;
+}
+
+// shard_sort -> boundary densities -> boundary forces (-> staging) ->
+// { exchange || interior densities -> apply -> interior forces }
+// ev[8] (optional): CUDA events at the stage boundaries, [5..6] around the exchange, [7] after the interior
+// densities (sph_shard_profile_step)
+int shard_sequence(SphCtx *c, cudaStream_t st, bool compute, bool wide, int64_t *kernels, cudaEvent_t *ev = nullptr) {
+    if (ev) cudaEventRecord(ev[0], st);
+    int rc = shard_sort(c, st, wide, kernels);
+    if (rc) return rc;
     if (ev) cudaEventRecord(ev[1], st);
     const dim3 pack_grid(blocks_for(c->P.halo_cap, 256), 2);
     if (compute) {
@@ -992,19 +1035,15 @@ int launch_shard_body_solve(SphCtx *c, cudaStream_t st, int64_t *kernels) {
 
 // One sharded WCSPH SPHBase.step() with dynamic solids (sph_shard_configure_bodies), in the order of launch_step +
 // launch_rigid_solve, on one stream and without overlap:
-//   plan -> classify + sort -> info -> solid-id slot map -> moving boundary volumes (owned + ghost layers 1-2)
+//   shard_sort -> solid-id slot map -> moving boundary volumes (owned + ghost layers 1-2)
 //   -> densities (owned + ghost layer 1) -> forces + integration of the owned fluid (no reaction scatter)
 //   -> reactions gathered onto the owned dynamic solids + their advection -> body-particle records -> all-gather ->
 //   k_rigid's solve + clamps on every rank -> clamps of the other dynamic solids -> pack the send ranges -> the record
 //   exchange
 int shard_bodies_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels) {
-    k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
-    *kernels += 1;
-    int rc = launch_neighbor_build(c, st, nullptr, kernels, /*move_acc=*/false);
+    int rc = shard_sort(c, st, wide, kernels);
     if (rc) return rc;
     const DevParams &P = c->P;
-    k_shard_info<<<1, 32, 0, st>>>(P, c->S, P.sgw + (wide ? 2 : 1), wide ? P.halo_cap : c->narrow_cap);
-    *kernels += 1;
     rc = launch_shard_solid_slots(c, st, kernels);
     if (rc) return rc;
     launch_pair_density(c, st, kernels, /*split_mode=*/0);
@@ -1074,24 +1113,6 @@ int sph_comm_set_transport(SphCtx *ctx, const SphTransport *t, int32_t rank, int
     return SPH_OK;
 }
 
-int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
-                        int32_t rebalance_every) {
-    if (!ctx) return SPH_E_ARG;
-    if (x_lo < 0 || x_hi > ctx->P.gx || ghost_layers < 1 || x_hi - x_lo < ghost_layers + 2)
-        return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
-    // Static solids travel in the records like fluid particles and never change; dynamic solids need moving boundary
-    // volumes one ghost layer deeper, reactions across a cut and a per-body reduction across ranks: the opt-in
-    // sph_shard_configure_bodies.
-    if (!ctx->bodies.empty() || (ctx->P.n_solid > 0 && ctx->has_dynamic_solids))
-        return fail(ctx, SPH_E_ARG, kShardStaticOnly);
-    if (!ctx->P.uniform_fluid)
-        return fail(ctx, SPH_E_ARG, "x-slab sharding needs a single fluid density (uniform fluid masses)");
-    if (halo_capacity < 1 || 2 * halo_capacity + ctx->P.n > ctx->n_max)
-        return fail(ctx, SPH_E_CAPACITY, "capacity: packed particles + 2 * halo_capacity receive slots exceed n_max");
-    if (rebalance_every < 0) return SPH_E_ARG;
-    return shard_setup(ctx, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, 0);
-}
-
 }  // extern "C"
 namespace {
 // The part of sph_shard_configure(_bodies) behind the argument checks: the shard buffer (n_body_particles > 0: with
@@ -1101,14 +1122,14 @@ int shard_setup(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, i
     const int32_t n_mine = ctx->P.n;
     drop_graphs(ctx);
     if (ctx->shard_buf) { cudaFree(ctx->shard_buf); ctx->shard_buf = nullptr; }
-    ctx->shard_bodies = false;
+    ctx->shard = ShardMode::Off; ctx->P.slab_on = 0;
     ctx->SL = make_shard_layout(halo_capacity, ctx->world, n_body_particles);
     CUDA_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->shard_buf), ctx->SL.total));
     CUDA_TRY(ctx, cudaMemset(ctx->shard_buf, 0, ctx->SL.total));
     int32_t sd[SD_INTS] = {0};
     sd[SD_N_LIVE] = n_mine; sd[SD_OWNED] = n_mine; sd[SD_SX0] = x_lo; sd[SD_SX1] = x_hi;
     CUDA_TRY(ctx, cudaMemcpy(ctx->shard_buf + ctx->SL.off_state, sd, sizeof(sd), cudaMemcpyHostToDevice));
-    ctx->P.slab_on = 1; ctx->P.sgw = ghost_layers; ctx->P.halo_cap = (int32_t)halo_capacity;
+    ctx->shard = ShardMode::Static; ctx->P.slab_on = 1; ctx->P.sgw = ghost_layers; ctx->P.halo_cap = (int32_t)halo_capacity;
     ctx->P.has_left = ctx->rank > 0; ctx->P.has_right = ctx->rank + 1 < ctx->world;
     ctx->P.rebalance_every = rebalance_every;
     ctx->narrow_cap = (int32_t)((halo_capacity * (ghost_layers + 1) + ghost_layers + 1) / (ghost_layers + 2));
@@ -1134,24 +1155,34 @@ int shard_setup(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, i
     return SPH_OK;
 }
 
-// sph_shard_configure_bodies (iisph = false: a WCSPH context) and sph_shard_configure_iisph_bodies (iisph = true: an
-// IISPH context): the same checks and set-up, only the solver asked for differs.
-int shard_configure_bodies(SphCtx *ctx, bool iisph, int32_t x_lo, int32_t x_hi, int32_t ghost_layers,
-                           int64_t halo_capacity, int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
-    if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
-    if (!iisph && ctx->iisph) return fail(ctx, SPH_E_ARG, kShardBodiesIisph);
-    if (iisph && !ctx->iisph) return fail(ctx, SPH_E_ARG, kShardIisphBodiesContext);
-    if (x_lo < 0 || x_hi > ctx->P.gx || x_hi - x_lo < ghost_layers + 2)
+// The slab arguments of both configure paths: the range (with ghost_layers >= 1, or >= 3 after it for bodies), then
+// `refusal` (may be NULL: why this path does not take the context), the fluid, the capacity and rebalance_every.
+int check_slab_args(SphCtx *ctx, bool bodies, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                    int32_t rebalance_every, const char *refusal) {
+    if (x_lo < 0 || x_hi > ctx->P.gx || (!bodies && ghost_layers < 1) || x_hi - x_lo < ghost_layers + 2)
         return fail(ctx, SPH_E_ARG, "slab must lie inside the grid and be at least ghost_layers + 2 cell layers wide");
-    if (ghost_layers < 3)
+    if (bodies && ghost_layers < 3)
         return fail(ctx, SPH_E_ARG, "dynamic solids need ghost_layers >= 3: the moving boundary volumes of the second "
                                     "ghost layer (read by the first layer's densities) sum solids of the third");
-    if (!iisph && ctx->P.dfsph) return fail(ctx, SPH_E_ARG, kShardBodiesWcsph);
+    if (refusal) return fail(ctx, SPH_E_ARG, refusal);
     if (!ctx->P.uniform_fluid)
         return fail(ctx, SPH_E_ARG, "x-slab sharding needs a single fluid density (uniform fluid masses)");
     if (halo_capacity < 1 || 2 * halo_capacity + ctx->P.n > ctx->n_max)
         return fail(ctx, SPH_E_CAPACITY, "capacity: packed particles + 2 * halo_capacity receive slots exceed n_max");
     if (rebalance_every < 0) return SPH_E_ARG;
+    return SPH_OK;
+}
+
+// sph_shard_configure_bodies (iisph = false: a WCSPH context) and sph_shard_configure_iisph_bodies (iisph = true: an
+// IISPH context): the same checks and set-up, only the solver asked for differs.
+int shard_configure_bodies(SphCtx *ctx, bool iisph, int32_t x_lo, int32_t x_hi, int32_t ghost_layers,
+                           int64_t halo_capacity, int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
+    if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
+    if ((ctx->solver == Solver::IISPH) != iisph)
+        return fail(ctx, SPH_E_ARG, iisph ? kShardIisphBodiesContext : kShardBodiesIisph);
+    if (int rc = check_slab_args(ctx, true, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every,
+                                 ctx->solver == Solver::DFSPH ? kShardBodiesWcsph : nullptr))
+        return rc;
     if (n_bodies > ctx->body_cap) return fail(ctx, SPH_E_CAPACITY, "more rigid bodies than the workspace was sized for");
     for (int b = 0; b < n_bodies; ++b) {
         const SphRigidBody &B = bodies[b];
@@ -1172,11 +1203,41 @@ int shard_configure_bodies(SphCtx *ctx, bool iisph, int32_t x_lo, int32_t x_hi, 
         ctx->err = why;
         return rc;
     }
-    ctx->shard_bodies = true;
+    ctx->shard = ShardMode::Bodies;
+    return SPH_OK;
+}
+
+// the exchange at the end of sequence q delivers the records plan kernel q + 1 works on; that one re-balances
+inline bool shard_wide(const SphCtx *c) {
+    const int64_t next_plan = c->shard_sequences + 1;
+    return c->P.rebalance_every > 0 && next_plan % c->P.rebalance_every == 0;
+}
+
+// The sharded step entry points: their mode checks, then nsteps sequences; sequence(wide) issues one (see shard_sort)
+template <typename Sequence>
+int run_shard_steps(SphCtx *ctx, int32_t nsteps, const Need &need, bool args_ok, Sequence sequence) {
+    if (int rc = require(ctx, need, args_ok)) return rc;
+    for (int s = 0; s < nsteps; ++s) {
+        if (int rc = sequence(shard_wide(ctx))) return rc;
+        ctx->shard_sequences += 1;
+    }
     return SPH_OK;
 }
 }  // namespace
 extern "C" {
+
+int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                        int32_t rebalance_every) {
+    if (!ctx) return SPH_E_ARG;
+    // Static solids travel in the records like fluid particles and never change; dynamic solids need moving boundary
+    // volumes one ghost layer deeper, reactions across a cut and a per-body reduction across ranks: the opt-in
+    // sph_shard_configure_bodies.
+    const bool dynamic = !ctx->bodies.empty() || (ctx->P.n_solid > 0 && ctx->has_dynamic_solids);
+    if (int rc = check_slab_args(ctx, false, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every,
+                                 dynamic ? kShardStaticOnly : nullptr))
+        return rc;
+    return shard_setup(ctx, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, 0);
+}
 
 int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                                int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
@@ -1189,18 +1250,8 @@ int sph_shard_configure_iisph_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, in
     return shard_configure_bodies(ctx, true, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, bodies, n_bodies);
 }
 
-// the exchange at the end of sequence q delivers the records plan kernel q + 1 works on; that one re-balances
-static inline bool shard_wide(const SphCtx *c) {
-    const int64_t next_plan = c->shard_sequences + 1;
-    return c->P.rebalance_every > 0 && next_plan % c->P.rebalance_every == 0;
-}
-
-#define REQUIRE_SHARD(ctx)                                                                              \
-    if (!(ctx)) return SPH_E_ARG;                                                                       \
-    if (!(ctx)->P.slab_on || !(ctx)->shard_buf) return fail((ctx), SPH_E_ARG, "sph_shard_configure was not called");
-
 int sph_shard_begin(SphCtx *ctx, void *stream) {
-    REQUIRE_SHARD(ctx);
+    if (int rc = require(ctx, Need().sharded())) return rc;
     ctx->shard_sequences = 0;
     int rc = shard_sequence(ctx, static_cast<cudaStream_t>(stream), /*compute=*/false, shard_wide(ctx), &ctx->launches);
     if (rc) return rc;
@@ -1210,49 +1261,37 @@ int sph_shard_begin(SphCtx *ctx, void *stream) {
 }
 
 int sph_halo_exchange(SphCtx *ctx, void *stream) {
-    REQUIRE_SHARD(ctx);
+    if (int rc = require(ctx, Need().sharded())) return rc;
     return shard_exchange(ctx, static_cast<cudaStream_t>(stream), /*wide=*/true);
 }
 
 int sph_shard_step(SphCtx *ctx, int32_t nsteps, void *stream) {
-    REQUIRE_SHARD(ctx);
-    if (nsteps < 0) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphShardStep);
-    if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_step is the WCSPH step; DFSPH contexts step with sph_shard_dfsph_step");
-    if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (ctx->shard_bodies) {  // always eager: SPH_SHARD_GRAPH does not apply
-        if (ctx->world != ctx->shard_world)
-            return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure_bodies: configure again");
-        for (int s = 0; s < nsteps; ++s) {
-            int rc = shard_bodies_sequence(ctx, st, shard_wide(ctx), &ctx->launches);
-            if (rc) return rc;
-            ctx->shard_sequences += 1;
-        }
-        return SPH_OK;
-    }
+    Need need = Need().shard_step(Solver::WCSPH, "sph_shard_step is the WCSPH step; DFSPH contexts step with "
+                                                 "sph_shard_dfsph_step");
+    // The world size sized the per-rank body tables of a body context; a static WCSPH context has no per-rank buffer
+    // and does not check it.  Body contexts always step eagerly: SPH_SHARD_GRAPH does not apply.
+    if (ctx && ctx->shard == ShardMode::Bodies)
+        return run_shard_steps(
+            ctx, nsteps, need.same_world("the transport's world size changed after sph_shard_configure_bodies: configure again"),
+            nsteps >= 0, [&](bool wide) { return shard_bodies_sequence(ctx, st, wide, &ctx->launches); });
     // Un-graphed launches are the DEFAULT here: nothing in a sharded step waits for the host any more, so the launches
     // run ahead of the device, and a graph replay -- whose two branches (exchange || interior forces) must both finish
     // before the next replay may start -- holds back the next step's first kernels, which un-graphed launches queue
     // behind the interior pass (not measured on H100s).  SPH_SHARD_GRAPH=1 replays the captured graph instead
     // (one graph per ping-pong parity and exchange width; pays off for small per-rank problems).
     static const bool eager = !(std::getenv("SPH_SHARD_GRAPH") && std::atoi(std::getenv("SPH_SHARD_GRAPH")) != 0);
-    for (int s = 0; s < nsteps; ++s) {
-        const bool wide = shard_wide(ctx);
+    return run_shard_steps(ctx, nsteps, need, nsteps >= 0, [&](bool wide) {
         auto issue = [&](cudaStream_t cs, int64_t *kernels) { return shard_sequence(ctx, cs, /*compute=*/true, wide, kernels); };
         // relaxed capture: NCCL may issue CUDA calls of its own while its send / recv kernels are being captured
-        int rc = eager ? issue(st, &ctx->launches)
-                       : replay_graph(ctx, st, ctx->graph_shard[ctx->parity][wide], 1, cudaStreamCaptureModeRelaxed,
-                                      "sharded graph", issue);
-        if (rc) return rc;
-        ctx->shard_sequences += 1;
-    }
-    return SPH_OK;
+        return eager ? issue(st, &ctx->launches)
+                     : replay_graph(ctx, st, ctx->graph_shard[ctx->parity][wide], 1, cudaStreamCaptureModeRelaxed,
+                                    "sharded graph", issue);
+    });
 }
 
 int sph_shard_info(SphCtx *ctx, int32_t *out16, uint64_t *out_sent, void *stream) {
-    REQUIRE_SHARD(ctx);
-    if (!out16) return SPH_E_ARG;
+    if (int rc = require(ctx, Need().sharded(), out16 != nullptr)) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int32_t sd[SD_INTS];
     uint32_t status = 0;
@@ -1275,7 +1314,7 @@ static_assert(sizeof(DumpHeader) == 16, "the dump header travels as 16 bytes");
 
 int sph_shard_dump(SphCtx *ctx, int32_t object_id, float *x, float *v, int64_t capacity, int64_t *rows_out,
                    uint32_t *status_out, void *stream) {
-    REQUIRE_SHARD(ctx);
+    if (int rc = require(ctx, Need().sharded())) return rc;
     if (!x || !v || !rows_out || !status_out || capacity < 0)
         return fail(ctx, SPH_E_ARG, "sph_shard_dump: x, v, rows_out and status_out must be non-null and capacity >= 0");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1375,14 +1414,10 @@ int sph_shard_dump(SphCtx *ctx, int32_t object_id, float *x, float *v, int64_t c
 }
 
 int sph_shard_profile_step(SphCtx *ctx, float *ms_out6, void *stream) {
-    REQUIRE_SHARD(ctx);
-    if (!ms_out6) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphShardStep);
-    if (ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_shard_profile_step times the WCSPH step");
-    if (ctx->shard_bodies)
-        return fail(ctx, SPH_E_ARG, "sph_shard_profile_step times the static-solid WCSPH step, not the step of a context "
-                                    "configured by sph_shard_configure_bodies");
-    if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
+    if (int rc = require(ctx, Need().shard_step(Solver::WCSPH, "sph_shard_profile_step times the WCSPH step").no_bodies(
+                                  "sph_shard_profile_step times the static-solid WCSPH step, not the step of a context "
+                                  "configured by sph_shard_configure_bodies"), ms_out6 != nullptr))
+        return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaEvent_t ev[8];
     for (int k = 0; k < 8; ++k) CUDA_TRY(ctx, cudaEventCreate(&ev[k]));
@@ -1403,26 +1438,19 @@ int sph_shard_profile_step(SphCtx *ctx, float *ms_out6, void *stream) {
 
 int sph_set_dfsph(SphCtx *ctx, int32_t enable) {
     if (!ctx) return SPH_E_ARG;
-    ctx->P.dfsph = enable ? 1 : 0;
-    ctx->iisph = false;
-    drop_graphs(ctx);
+    set_solver(ctx, enable ? Solver::DFSPH : Solver::WCSPH);
     return SPH_OK;
 }
 
 int sph_set_iisph(SphCtx *ctx, int32_t enable) {
-    if (!ctx) return SPH_E_ARG;
-    if (enable && ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphAfterConfigure);
-    if (!enable && !ctx->iisph) return SPH_OK;  // not in IISPH mode: a DFSPH or WCSPH context stays as it is
-    ctx->P.dfsph = enable ? 1 : 0;
-    ctx->iisph = enable != 0;
-    drop_graphs(ctx);
+    if (int rc = require(ctx, Need().unsharded(enable ? kIisphAfterConfigure : nullptr))) return rc;
+    if (!enable && ctx->solver != Solver::IISPH) return SPH_OK;  // not in IISPH mode: a DFSPH or WCSPH context stays
+    set_solver(ctx, enable ? Solver::IISPH : Solver::WCSPH);
     return SPH_OK;
 }
 
 int sph_dfsph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
-    if (!ctx) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
-    if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called");
+    if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph))) return rc;
     const DevParams &P = ctx->P;
     if (P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1601,7 +1629,7 @@ int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double et
 // constants in, counts out.  The exchanges run only on a sharded context: v* after predict_velocity (read by
 // k_iisph_predict), aux after k_iisph_predict (the warm-start p / rho^2 the first sweep reads), then the two of every
 // sweep.  compute_pressure_forces reads the aux words the converged sweep sent; nothing reads a ghost value after it.
-// Sharded with dynamic solids (c->shard_bodies): compute_pressure_forces runs without its reaction scatter (it would add
+// Sharded with dynamic solids (ShardMode::Bodies): compute_pressure_forces runs without its reaction scatter (it would add
 // the reactions a second time, and onto ghost copies), the first ghost layer's final pressures arrive in one more
 // message (DX_MISC) and k_iisph_shard_reactions gathers the reactions onto the owned dynamic solids before the advect.
 int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n_grid, int64_t *kernels) {
@@ -1625,7 +1653,7 @@ int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n
                           kernels);
     if (rc) return rc;
     io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-    if (c->shard_bodies) {
+    if (c->shard == ShardMode::Bodies) {
         k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, c->S, nullptr);
         *kernels += 1;
         rc = shard_dfsph_exchange(c, st, DX_MISC, nullptr, false, kernels);
@@ -1715,24 +1743,22 @@ int single_step(SphCtx *ctx, cudaStream_t st, Substep substep) {
 
 // One sharded SPHBase.step() of a solver whose substep launches itself (DFSPH, IISPH; no overlap of the exchanges with
 // computation):
-//   plan -> classify + sort -> info -> DX ranges -> ghost alignment [-> solid-id slot map -> moving boundary volumes]
+//   shard_sort -> DX ranges -> ghost alignment [-> solid-id slot map -> moving boundary volumes]
 //   -> substep(n_grid) on owned records + ghosts [-> body all-gather + solve -> clamps of the other dynamic solids]
 //   -> clamp (owned fluid) -> pack the send ranges -> the record exchange that feeds the next step's classification
-// [..]: contexts with dynamic solids only (c->shard_bodies; IISPH, sph_shard_configure_iisph_bodies).
+// [..]: body contexts only (ShardMode::Bodies; IISPH, sph_shard_configure_iisph_bodies).
 template <typename Substep>
 int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels, Substep substep) {
-    k_shard_plan<<<1, 32, 0, st>>>(c->P, c->S);
-    *kernels += 1;
-    int rc = launch_neighbor_build(c, st, nullptr, kernels, /*move_acc=*/false);
+    const bool bodies = c->shard == ShardMode::Bodies;
+    int rc = shard_sort(c, st, wide, kernels);
     if (rc) return rc;
     const DevParams &P = c->P;
-    k_shard_info<<<1, 32, 0, st>>>(P, c->S, P.sgw + (wide ? 2 : 1), wide ? P.halo_cap : c->narrow_cap);
     k_dfsph_shard_ranges<<<1, 32, 0, st>>>(P, c->S, shard_dx(c), c->align_cap, c->sweep_cap);
-    *kernels += 2;
+    *kernels += 1;
     CUDA_TRY(c, cudaGetLastError());
     rc = shard_dfsph_exchange(c, st, DX_ALIGN, nullptr, false, kernels);
     if (rc) return rc;
-    if (c->shard_bodies) { rc = launch_shard_solid_slots(c, st, kernels); if (rc) return rc; }
+    if (bodies) { rc = launch_shard_solid_slots(c, st, kernels); if (rc) return rc; }
     // The step waits on the host once per batch of sweeps anyway; one more short wait here for the live count lets
     // every substep launch cover [0, n_live) -- owned records and ghosts -- instead of the whole capacity.
     int32_t n_live = 0;
@@ -1742,7 +1768,7 @@ int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels
     rc = substep(n_grid);
     if (rc) return rc;
     // solve_rigid_body(), enforce_boundary_3D(fluid) (sph_base.py:270-271)
-    if (c->shard_bodies) { rc = launch_shard_body_solve(c, st, kernels); if (rc) return rc; }
+    if (bodies) { rc = launch_shard_body_solve(c, st, kernels); if (rc) return rc; }
     k_enforce_boundary<<<blocks_for(n_grid, 256), 256, 0, st>>>(P, c->S, /*particle_type=*/1);
     // the advanced records of the send ranges -> staging, then the exchange the next step classifies
     k_shard_apply<<<dim3(blocks_for(P.halo_cap, 256), 2), 256, 0, st>>>(P, c->S, /*copy_all=*/1);
@@ -1756,11 +1782,8 @@ extern "C" {
 
 int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double eta, float offset, int64_t n_fluid,
                     int32_t first_batch, int32_t *iterations_out, int32_t *sweeps_out, double *avg_err_out, void *stream) {
-    if (!ctx || (mode != 0 && mode != 1) || n_fluid < 1) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
-    if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called");
-    if (!ctx->built || !ctx->list_valid)
-        return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run sph_neighbor_build and op 0 (compute_densities) first");
+    if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph).fresh_lists(), (mode == 0 || mode == 1) && n_fluid >= 1))
+        return rc;
     DfsphCtrl h{};
     int rc = dfsph_solve_loop(ctx, mode, max_iterations, eta, offset, n_fluid, first_batch, &h,
                               static_cast<cudaStream_t>(stream), ctx->P.n, &ctx->launches);
@@ -1772,10 +1795,9 @@ int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double et
 }
 
 int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) {
-    if (!ctx || !io || nsteps < 0 || io->n_fluid < 1) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphContext);
-    if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called");
-    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, "this context is sharded: step it with sph_shard_dfsph_step");
+    const char *sharded = "this context is sharded: step it with sph_shard_dfsph_step";
+    if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph).unsharded(sharded), io && nsteps >= 0 && io->n_fluid >= 1))
+        return rc;
     if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int s = 0; s < nsteps; ++s) {
@@ -1786,9 +1808,7 @@ int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) 
 }
 
 int sph_iisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
-    if (!ctx) return SPH_E_ARG;
-    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
-    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSharded);
+    if (int rc = require(ctx, Need().runs(Solver::IISPH, kNoIisph).unsharded(kIisphSharded))) return rc;
     const DevParams &P = ctx->P;
     if (P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1835,11 +1855,9 @@ int sph_iisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream
 
 int sph_iisph_solve(SphCtx *ctx, int32_t max_iterations, float omega, double eta, int64_t n_fluid, int32_t first_batch,
                     int32_t *iterations_out, double *avg_err_out, void *stream) {
-    if (!ctx || n_fluid < 1 || max_iterations < 1) return SPH_E_ARG;
-    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
-    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSharded);
-    if (!ctx->built || !ctx->list_valid)
-        return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run sph_neighbor_build and op 0 (compute_densities) first");
+    if (int rc = require(ctx, Need().runs(Solver::IISPH, kNoIisph).unsharded(kIisphSharded).fresh_lists(),
+                         n_fluid >= 1 && max_iterations >= 1))
+        return rc;
     DfsphCtrl h{};
     int rc = iisph_solve_loop(ctx, max_iterations, omega, eta, n_fluid, first_batch, &h, static_cast<cudaStream_t>(stream),
                               ctx->P.n, &ctx->launches);
@@ -1850,9 +1868,9 @@ int sph_iisph_solve(SphCtx *ctx, int32_t max_iterations, float omega, double eta
 }
 
 int sph_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream) {
-    if (!ctx || !io || nsteps < 0 || io->n_fluid < 1 || io->max_iterations < 1) return SPH_E_ARG;
-    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
-    if (ctx->P.slab_on) return fail(ctx, SPH_E_ARG, kIisphSharded);
+    if (int rc = require(ctx, Need().runs(Solver::IISPH, kNoIisph).unsharded(kIisphSharded),
+                         io && nsteps >= 0 && io->n_fluid >= 1 && io->max_iterations >= 1))
+        return rc;
     if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int s = 0; s < nsteps; ++s) {
@@ -1863,8 +1881,7 @@ int sph_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream) 
 }
 
 int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) {
-    if (!ctx) return SPH_E_ARG;
-    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called");
+    if (int rc = require(ctx, Need().runs(Solver::IISPH, kNoIisph))) return rc;
     if (ctx->P.n == 0) return SPH_OK;
     k_iisph_read<<<blocks_for(ctx->P.n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S, a_ii, s, ap);
     ctx->launches += 1;
@@ -1873,41 +1890,23 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) 
 }
 
 int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) {
-    REQUIRE_SHARD(ctx);
-    if (!io || nsteps < 0 || io->n_fluid < 1) return SPH_E_ARG;
-    if (ctx->iisph) return fail(ctx, SPH_E_ARG, kIisphShardStep);  // sph_set_iisph sets P.dfsph too
-    if (!ctx->P.dfsph) return fail(ctx, SPH_E_ARG, "sph_set_dfsph(1) was not called: WCSPH contexts step with sph_shard_step");
-    if (ctx->shard_bodies) return fail(ctx, SPH_E_ARG, kShardBodiesWcsph);
-    if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
-    if (ctx->world != ctx->shard_world)
-        return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure: configure again");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int s = 0; s < nsteps; ++s) {
-        int rc = shard_dfsph_sequence(ctx, st, shard_wide(ctx), &ctx->launches, [&](int64_t n_grid) {
-            return launch_dfsph_substep(ctx, st, io, n_grid, &ctx->launches);
-        });
-        if (rc) return rc;
-        ctx->shard_sequences += 1;
-    }
-    return SPH_OK;
+    const char *wcsph = "sph_set_dfsph(1) was not called: WCSPH contexts step with sph_shard_step";
+    Need need = Need().shard_step(Solver::DFSPH, wcsph).no_bodies(kShardBodiesWcsph).same_world(kWorldChanged);
+    return run_shard_steps(ctx, nsteps, need, io && nsteps >= 0 && io->n_fluid >= 1, [&](bool wide) {
+        return shard_dfsph_sequence(ctx, st, wide, &ctx->launches,
+                                    [&](int64_t n_grid) { return launch_dfsph_substep(ctx, st, io, n_grid, &ctx->launches); });
+    });
 }
 
 int sph_shard_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream) {
-    REQUIRE_SHARD(ctx);
-    if (!io || nsteps < 0 || io->n_fluid < 1 || io->max_iterations < 1) return SPH_E_ARG;
-    if (!ctx->iisph) return fail(ctx, SPH_E_ARG, "sph_set_iisph(1) was not called before sph_shard_configure");
-    if (!ctx->shard_begun) return fail(ctx, SPH_E_ARG, "sph_shard_begin was not called");
-    if (ctx->world != ctx->shard_world)
-        return fail(ctx, SPH_E_ARG, "the transport's world size changed after sph_shard_configure: configure again");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int s = 0; s < nsteps; ++s) {
-        int rc = shard_dfsph_sequence(ctx, st, shard_wide(ctx), &ctx->launches, [&](int64_t n_grid) {
-            return launch_iisph_substep(ctx, st, io, n_grid, &ctx->launches);
-        });
-        if (rc) return rc;
-        ctx->shard_sequences += 1;
-    }
-    return SPH_OK;
+    Need need = Need().shard_step(Solver::IISPH, "sph_set_iisph(1) was not called before sph_shard_configure");
+    return run_shard_steps(ctx, nsteps, need.same_world(kWorldChanged),
+                           io && nsteps >= 0 && io->n_fluid >= 1 && io->max_iterations >= 1, [&](bool wide) {
+        return shard_dfsph_sequence(ctx, st, wide, &ctx->launches,
+                                    [&](int64_t n_grid) { return launch_iisph_substep(ctx, st, io, n_grid, &ctx->launches); });
+    });
 }
 
 int sph_shard_transport_stats(SphCtx *ctx, uint64_t *out2) {
