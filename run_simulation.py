@@ -111,10 +111,10 @@ def run_sharded(config, scene_name, frames, device, transport=None, quiet=False,
 
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
-    dynamic = any(o.get("isDynamic") for o in list(config.get_rigid_bodies()) + list(config.get_rigid_blocks()))
     try:
         sim, n_total = slab.build_sharded(_resolved_scene(config), rank, world, device, transport=transport,
-                                          dynamic_solids=dynamic, iisph=iisph, iisph_bodies=iisph_bodies)
+                                          dynamic_solids=slab.scene_has_dynamic_solids(config), iisph=iisph,
+                                          iisph_bodies=iisph_bodies)
     except NotImplementedError as exc:
         raise SystemExit(f"{scene_name}: {exc}") from exc
     substeps = config.get_cfg("numberOfStepsPerRenderUpdate")

@@ -22,18 +22,18 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
 * Static solids (``RigidBlocks`` / ``RigidBodies`` with ``isDynamic: false``) ride the record exchange like fluid
   particles and never change.  Their boundary volumes depend on solid neighbours that may sit across a cut, so
   ``build_sharded`` computes them once, before the first exchange, over the whole scene exactly as the single engine
-  does (``startup_boundary_volumes``).
+  does (``startup_state``).
 * Dynamic solids (shape-matched ``RigidBodies`` and advected ``RigidBlocks`` with ``isDynamic: true``) are opt-in,
   WCSPH only: ``build_sharded(..., dynamic_solids=True)`` configures the engine with ``sph_shard_configure_bodies``.
   Each rank then keeps 3 ghost layers (a moving solid's boundary volume in the second ghost layer sums solids of the
   third), gathers the fluid's reactions onto the dynamic solids it owns (fluid owned across a cut included), and
   solves every body on every rank with the single engine's shape-matching reduction over an all-gather of all body
   particles' records: cm and R are bit-identical on every rank and equal to the single engine's for the same particle
-  positions (``ShardedSimulation.body_state``).  The bodies' rest centres of mass are computed
-  over the whole scene exactly as the single engine computes them (``startup_rest_cms``).  That step is launched
-  eagerly, without overlap; ``SPH_SHARD_GRAPH`` does not apply.  Without the flag, and for DFSPH in any case, dynamic
-  solids are refused (``STATIC_SOLIDS_ONLY`` / ``DYNAMIC_SOLIDS_WCSPH_ONLY``): the DFSPH pressure sweeps scatter the
-  reactions in every sweep, which would need a reaction exchange per sweep.
+  positions (``ShardedSimulation.body_state``).  The bodies' rest centres of mass are computed over the whole scene
+  exactly as the single engine computes them, in the same pass as the boundary volumes (``startup_state``).  That
+  step is launched eagerly, without overlap; ``SPH_SHARD_GRAPH`` does not apply.  Without the flag, and for DFSPH in
+  any case, dynamic solids are refused (``STATIC_SOLIDS_ONLY`` / ``DYNAMIC_SOLIDS_WCSPH_ONLY``): the DFSPH pressure
+  sweeps scatter the reactions in every sweep, which would need a reaction exchange per sweep.
 * IISPH scenes (``simulationMethod: 3``) are opt-in: ``build_sharded(..., iisph=True)`` (``run_simulation.py --gpus N
   --shard-iisph``); without it they are refused (``IISPH_SINGLE_GPU``).  They step through ``sph_shard_iisph_step``,
   the DFSPH step's shape with IISPH's substep: the once-per-step ghost alignment, the predicted velocities and the
@@ -58,6 +58,8 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
+import enum
 import json
 import os
 import time
@@ -90,14 +92,72 @@ DYNAMIC_SOLIDS_IISPH = ("x-slab sharding of dynamic solids is WCSPH only: dynami
                         "--shard-iisph-bodies (sharded IISPH otherwise runs fluid and static solids)")
 
 
+class Solver(enum.IntEnum):
+    """The solvers a scene can shard with, valued by their ``simulationMethod``."""
+    WCSPH = 0
+    IISPH = 3
+    DFSPH = 4
+
+
+@dataclasses.dataclass(frozen=True)
+class ShardMode:
+    """What a sharded run is: its solver, and whether it shards dynamic solids (``bodies``: 3 ghost layers, reactions
+    gathered across cuts, bodies solved on every rank)."""
+    solver: Solver
+    bodies: bool
+
+    @property
+    def ghost_layers(self):
+        return GHOST_LAYERS_BODIES if self.bodies else GHOST_LAYERS
+
+    @property
+    def send_layers(self):
+        return SEND_LAYERS_BODIES if self.bodies else SEND_LAYERS
+
+
+def scene_has_dynamic_solids(cfg):
+    """Whether any rigid body or rigid block of the scene is dynamic."""
+    return any(o.get("isDynamic") for o in list(cfg.get_rigid_bodies() or []) + list(cfg.get_rigid_blocks() or []))
+
+
+def shard_mode(method, scene_dynamic, dynamic_solids=False, iisph=False, iisph_bodies=False):
+    """The ``ShardMode`` of ``build_sharded``'s opt-ins on a scene of ``simulationMethod`` ``method`` that has dynamic
+    solids or not (``scene_dynamic``); raises when that mode is not sharded.  ``iisph_bodies`` implies ``iisph`` and
+    ``dynamic_solids``."""
+    if iisph_bodies and method != 3:
+        raise ValueError(f"iisph_bodies=True shards an IISPH scene (simulationMethod 3) with dynamic solids, not "
+                         f"simulationMethod {method}")
+    if method == 3 and not (iisph or iisph_bodies):
+        raise NotImplementedError(IISPH_SINGLE_GPU)
+    if method not in (0, 3, 4):
+        raise NotImplementedError(f"x-slab sharding runs WCSPH (0), DFSPH (4) and IISPH (3) scenes, not "
+                                  f"simulationMethod {method}")
+    if iisph and method != 3:
+        raise ValueError(f"iisph=True shards an IISPH scene (simulationMethod 3), not simulationMethod {method}")
+    if iisph and not iisph_bodies and (dynamic_solids or scene_dynamic):
+        raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
+    bodies = dynamic_solids or iisph_bodies
+    if bodies and method == 4:
+        raise NotImplementedError(DYNAMIC_SOLIDS_WCSPH_ONLY)
+    return ShardMode(Solver(method), bool(bodies))
+
+
+def scene_geometry(cfg):
+    """(h, grid_num, m_V0, domain size) of a scene as ``ParticleSystem`` derives them; m_V0 in float32, the value the
+    engine's fields hold."""
+    ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
+    radius = cfg.get_cfg("particleRadius")
+    h = radius * 4.0
+    return h, np.ceil(ds / h).astype(int), np.float32(0.8 * (2 * radius) ** 3), ds
+
+
 def scene_params(cfg):
     """The engine constants of a scene, as ``ParticleSystem`` derives them before a solver overrides any."""
     from . import engine as _engine
-    ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
-    radius = cfg.get_cfg("particleRadius")
-    grid_num = np.ceil(ds / (radius * 4.0)).astype(int)
-    return _engine.make_params(3, grid_num, radius, cfg.get_cfg("density0"), cfg.get_cfg("stiffness"),
-                               cfg.get_cfg("exponent"), cfg.get_cfg("timeStepSize"), cfg.get_cfg("gravitation"), ds)
+    _, grid_num, _, ds = scene_geometry(cfg)
+    return _engine.make_params(3, grid_num, cfg.get_cfg("particleRadius"), cfg.get_cfg("density0"),
+                               cfg.get_cfg("stiffness"), cfg.get_cfg("exponent"), cfg.get_cfg("timeStepSize"),
+                               cfg.get_cfg("gravitation"), ds)
 
 
 def solid_ids(arrays):
@@ -129,37 +189,6 @@ def field_tensors(arrays, n, m_V0, device):
     }
 
 
-def startup_boundary_volumes(cfg, arrays, device):
-    """m_V of every particle of the whole scene after ``SPHBase.initialize()``: the single engine's start-up boundary
-    volumes (``compute_static_boundary_volume`` then ``compute_moving_boundary_volume``), computed by the same kernels
-    on the same packed scene, hence bit-identical to them; fluid particles keep m_V0.  ``arrays`` must hold
-    ``solid_id``.  Every rank runs this on the whole scene, so every rank holds the same value for every solid."""
-    from . import engine as _engine
-    n = len(arrays["material"])
-    sid = np.asarray(arrays["solid_id"])
-    n_solid = int((sid >= 0).sum())
-    m_V0 = float(np.float32(0.8 * (2 * cfg.get_cfg("particleRadius")) ** 3))
-    out = np.full(n, np.float32(m_V0), np.float32)
-    if n_solid == 0:
-        return out
-    eng = _engine.Engine(scene_params(cfg), n_max=n, n_solid=n_solid, n_bodies=0, device=device)
-    try:
-        f = field_tensors(arrays, n, m_V0, device)
-        eng.pack(f, n, n_solid, bool((np.asarray(arrays["is_dynamic"])[sid >= 0] != 0).any()))
-        eng.neighbor_build()
-        eng.boundary_volume(0)
-        eng.boundary_volume(1)
-        eng.unpack(f)  # sorted order; solid_id maps it back
-        got_sid, got_mV = f["solid_id"].cpu().numpy(), f["m_V"].cpu().numpy()
-    finally:
-        eng.close()
-    by_sid = np.empty(n_solid, np.float32)
-    s = got_sid >= 0
-    by_sid[got_sid[s]] = got_mV[s]
-    out[sid >= 0] = by_sid[sid[sid >= 0]]
-    return out
-
-
 def dynamic_bodies(cfg, arrays):
     """The shape-matched bodies as the single engine registers them (``ParticleSystem._prepare_solids``): every
     dynamic ``RigidBodies`` object in object-id order, with the range of its global solid ids (``solid_ids``).
@@ -175,22 +204,40 @@ def dynamic_bodies(cfg, arrays):
     return out
 
 
-def startup_rest_cms(cfg, arrays, bodies, device):
-    """Each body's rest centre of mass as ``SPHBase.compute_rigid_rest_cm`` computes it at start-up: the same kernel
-    on the same packed scene (the sum runs in solid-id order), hence bit-identical to the single engine's."""
+def startup_state(cfg, arrays, bodies, device):
+    """The whole scene's start-up state as the single engine's ``SPHBase.initialize()`` leaves it, computed by the
+    same kernels on the same packed scene, hence bit-identical to it.  Returns (m_V of every particle, the rest centre
+    of mass of each of ``bodies`` [(object_id, solid_begin, solid_end)]).  m_V holds the boundary volumes of
+    ``compute_static_boundary_volume`` then ``compute_moving_boundary_volume``; fluid particles keep m_V0.  The rest
+    centres of mass are ``compute_rigid_rest_cm``'s, summed in solid-id order.  They do not depend on m_V (a solid's
+    mass is m_V0 * density), so computing them first changes neither result.  ``arrays`` must hold ``solid_id`` and at
+    least one solid.  Every rank runs this on the whole scene, so every rank holds the same values."""
     from . import engine as _engine
     n = len(arrays["material"])
     sid = np.asarray(arrays["solid_id"])
-    n_solid = int((sid >= 0).sum())
-    m_V0 = float(np.float32(0.8 * (2 * cfg.get_cfg("particleRadius")) ** 3))
+    solid = sid >= 0
+    n_solid = int(solid.sum())
+    m_V0 = float(scene_geometry(cfg)[2])
     eng = _engine.Engine(scene_params(cfg), n_max=n, n_solid=n_solid, n_bodies=len(bodies), device=device)
     try:
-        eng.pack(field_tensors(arrays, n, m_V0, device), n, n_solid, True)
-        eng.set_rigid_bodies([(o, b0, b1, [np.nan] * 3) for o, b0, b1 in bodies])
+        f = field_tensors(arrays, n, m_V0, device)
+        eng.pack(f, n, n_solid, bool((np.asarray(arrays["is_dynamic"])[solid] != 0).any()))
+        if bodies:
+            eng.set_rigid_bodies([(o, b0, b1, [np.nan] * 3) for o, b0, b1 in bodies])
         eng.neighbor_build()
-        return [eng.compute_com(b).cpu().numpy().astype(np.float32) for b in range(len(bodies))]
+        rest_cms = [eng.compute_com(b).cpu().numpy().astype(np.float32) for b in range(len(bodies))]
+        eng.boundary_volume(0)
+        eng.boundary_volume(1)
+        eng.unpack(f)  # sorted order; solid_id maps it back
+        got_sid, got_mV = f["solid_id"].cpu().numpy(), f["m_V"].cpu().numpy()
     finally:
         eng.close()
+    by_sid = np.empty(n_solid, np.float32)
+    s = got_sid >= 0
+    by_sid[got_sid[s]] = got_mV[s]
+    m_V = np.full(n, np.float32(m_V0), np.float32)
+    m_V[solid] = by_sid[sid[solid]]
+    return m_V, rest_cms
 
 
 def plan_slabs(layer_counts, world, min_width=SEND_LAYERS + 1):
@@ -270,33 +317,23 @@ class GlooTransport:
 class ShardedSimulation:
     """This rank's share of a sharded scene: a CUDA engine in slab mode + the library's halo exchange."""
 
-    def __init__(self, cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, uniform_hint, group=None,
-                 rebalance_every=8, transport=None, n_fluid=None, n_solid=0, bodies=None, iisph_bodies=False):
-        """``mine``: this rank's initial particles (numpy arrays in the reference's field layout); with solids also
-        ``solid_id`` (global ids, ``solid_ids``) and ``m_V`` (start-up boundary volumes, ``startup_boundary_volumes``).
-        ``n_solid``: the solid count of the WHOLE scene (sizes the solid-id slot map).  ``bodies`` (dynamic solids;
-        WCSPH, or IISPH with ``iisph_bodies=True``): [(object_id, solid_begin, solid_end, rest_cm)] of the whole scene
-        (``dynamic_bodies``, ``startup_rest_cms``), an empty list for advected rigid blocks only; None refuses dynamic
-        solids."""
+    def __init__(self, cfg, mode, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, uniform_hint, group=None,
+                 rebalance_every=8, transport=None, n_fluid=None, n_solid=0, bodies=None):
+        """``mode``: the run's ``ShardMode`` (``shard_mode``).  ``mine``: this rank's initial particles (numpy arrays in
+        the reference's field layout); with solids also ``solid_id`` (global ids, ``solid_ids``) and ``m_V`` (start-up
+        boundary volumes, ``startup_state``).  ``n_solid``: the solid count of the WHOLE scene (sizes the solid-id
+        slot map).  ``bodies`` (a mode with bodies): [(object_id, solid_begin, solid_end, rest_cm)] of the whole scene
+        (``dynamic_bodies``, ``startup_state``), an empty list for advected rigid blocks only; None otherwise."""
         from . import engine as _engine
-        self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
-        self.dfsph = cfg.get_cfg("simulationMethod") == 4
-        self.iisph = cfg.get_cfg("simulationMethod") == 3
-        if (self.dfsph or self.iisph) and not n_fluid:
+        self.cfg, self.mode, self.rank, self.world, self.group = cfg, mode, rank, world, group
+        if mode.solver is not Solver.WCSPH and not n_fluid:
             raise ValueError("a sharded DFSPH or IISPH scene needs n_fluid, the fluid particle count of ALL ranks")
         self.device = torch.device(device)
         self.slabs0 = [tuple(int(v) for v in s_) for s_ in slabs]
-        ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
-        radius = cfg.get_cfg("particleRadius")
-        self.h = radius * 4.0
-        self.grid_num = np.ceil(ds / self.h).astype(int)
-        self.m_V0 = float(np.float32(0.8 * (2 * radius) ** 3))
+        self.h, self.grid_num, m_V0, _ = scene_geometry(cfg)
+        self.m_V0 = float(m_V0)
         self.n_cap, self.halo_cap, self.n_solid = int(n_cap), int(halo_cap), int(n_solid)
         self.bodies = None if bodies is None else list(bodies)
-        if self.bodies is not None and self.dfsph:
-            raise NotImplementedError(DYNAMIC_SOLIDS_WCSPH_ONLY)
-        if self.bodies is not None and self.iisph and not iisph_bodies:
-            raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
         self.eng = _engine.Engine(scene_params(cfg), n_max=self.n_cap, n_solid=self.n_solid,
                                   n_bodies=len(self.bodies or []), device=self.device)
         e = self.eng
@@ -304,12 +341,13 @@ class ShardedSimulation:
         self.last_iterations_v = self.last_iterations = 0
         self._io = None
         self.last_avg_err = 0.0
-        if self.dfsph:
+        # the solver is set before sph_shard_configure: the library refuses the switch on a sharded context
+        if mode.solver is Solver.DFSPH:
             e.set_dfsph(True)
             from .DFSPH import dfsph_step_io
             self._io = dfsph_step_io(float(cfg.get_cfg("timeStepSize")), float(cfg.get_cfg("density0")), n_fluid)
-        elif self.iisph:
-            e.set_iisph(True)  # before sph_shard_configure: the library refuses it on a sharded context
+        elif mode.solver is Solver.IISPH:
+            e.set_iisph(True)
             from .IISPH import iisph_step_io
             self._io = iisph_step_io(n_fluid)
         # ---- transport: NCCL inside the library (its own communicator), or a caller-supplied one (tests) ----
@@ -329,17 +367,17 @@ class ShardedSimulation:
         else:
             e._check(e.lib.sph_comm_set_transport(e.ctx, None, 0, 1), "sph_comm_set_transport")
         lo, hi = self.slabs0[rank]
-        if self.bodies is None:
-            e._check(e.lib.sph_shard_configure(e.ctx, lo, hi, GHOST_LAYERS, self.halo_cap, int(rebalance_every)),
-                     "sph_shard_configure")
+        args = (e.ctx, lo, hi, mode.ghost_layers, self.halo_cap, int(rebalance_every))
+        if not mode.bodies:
+            name = "sph_shard_configure"
         else:
             table = (_lib.SphRigidBody * max(1, len(self.bodies)))()
             for i, (oid, b0, b1, rest_cm) in enumerate(self.bodies):
                 table[i].object_id, table[i].solid_begin, table[i].solid_end = int(oid), int(b0), int(b1)
                 table[i].rest_cm = (C.c_float * 3)(*[float(v) for v in rest_cm])
-            name = "sph_shard_configure_iisph_bodies" if self.iisph else "sph_shard_configure_bodies"
-            e._check(getattr(e.lib, name)(e.ctx, lo, hi, GHOST_LAYERS_BODIES, self.halo_cap, int(rebalance_every),
-                                          table, len(self.bodies)), name)
+            name = "sph_shard_configure_iisph_bodies" if mode.solver is Solver.IISPH else "sph_shard_configure_bodies"
+            args += (table, len(self.bodies))
+        e._check(getattr(e.lib, name)(*args), name)
         e._check(e.lib.sph_shard_begin(e.ctx, e._stream()), "sph_shard_begin")
         self.steps_done = 0
         # the scene's objects and per-object particle counts (build_sharded sets them; dump() sizes rank 0's buffers
@@ -350,14 +388,19 @@ class ShardedSimulation:
     def _load(self, arrays, n, uniform_hint):
         """Pack this rank's initial particles (numpy arrays in the reference's field layout)."""
         solid = np.asarray(arrays["material"]) != 1
-        dynamic = self.bodies is not None
-        if not dynamic and bool((solid & (np.asarray(arrays["is_dynamic"]) != 0)).any()):
-            raise NotImplementedError(STATIC_SOLIDS_ONLY)
         if solid.any() and ("solid_id" not in arrays or "m_V" not in arrays):
             raise ValueError("solid particles need their global solid_id and start-up m_V (see build_sharded)")
         f = field_tensors(arrays, n, self.m_V0, self.device)
-        self.eng.pack(f, n, self.n_solid, dynamic, uniform_hint=uniform_hint)
+        self.eng.pack(f, n, self.n_solid, self.mode.bodies, uniform_hint=uniform_hint)
         self.synchronize()  # the temporaries above may be freed now
+
+    @property
+    def dfsph(self):
+        return self.mode.solver is Solver.DFSPH
+
+    @property
+    def iisph(self):
+        return self.mode.solver is Solver.IISPH
 
     # ---- stepping --------------------------------------------------------------------------------------
     def step(self, n=1):
@@ -365,14 +408,12 @@ class ShardedSimulation:
         ``last_avg_err``) are those of the last step, the same on every rank; IISPH: ``last_iterations`` /
         ``last_avg_err`` (pressure sweeps and their last average error), the same on every rank.  Both wait on the
         device once per batch of Jacobi sweeps."""
-        e = self.eng
-        if self.dfsph:
-            io = self._io
+        e, io = self.eng, self._io
+        if self.mode.solver is Solver.DFSPH:
             e._check(e.lib.sph_shard_dfsph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_dfsph_step")
             self.last_iterations_v, self.last_iterations = int(io.iterations_v), int(io.iterations)
             self.last_avg_err_v, self.last_avg_err = float(io.avg_err_v), float(io.avg_err)
-        elif self.iisph:
-            io = self._io  # first_batch: in, the previous step's sweeps; out, this step's
+        elif self.mode.solver is Solver.IISPH:  # io.first_batch: in, the previous step's sweeps; out, this step's
             e._check(e.lib.sph_shard_iisph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_iisph_step")
             self.last_iterations, self.last_avg_err = int(io.iterations), float(io.avg_err)
         else:
@@ -516,62 +557,40 @@ def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1
     from .scene import assemble_particles
 
     cfg = SimConfig(scene_dict)
-    method = cfg.get_cfg("simulationMethod")
-    if iisph_bodies and method != 3:
-        raise ValueError(f"iisph_bodies=True shards an IISPH scene (simulationMethod 3) with dynamic solids, not "
-                         f"simulationMethod {method}")
-    if method == 3 and not (iisph or iisph_bodies):
-        raise NotImplementedError(IISPH_SINGLE_GPU)
-    if method not in (0, 3, 4):
-        raise NotImplementedError(f"x-slab sharding runs WCSPH (0), DFSPH (4) and IISPH (3) scenes, not "
-                                  f"simulationMethod {method}")
-    if iisph and method != 3:
-        raise ValueError(f"iisph=True shards an IISPH scene (simulationMethod 3), not simulationMethod {method}")
-    if iisph_bodies:
-        iisph = dynamic_solids = True
-    elif iisph and (dynamic_solids or any(o.get("isDynamic") for o in
-                                        list(cfg.get_rigid_bodies() or []) + list(cfg.get_rigid_blocks() or []))):
-        raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
-    radius = cfg.get_cfg("particleRadius")
-    h = radius * 4.0
-    arrays, object_collection, _, counts = assemble_particles(cfg, 3, 2 * radius)
+    mode = shard_mode(cfg.get_cfg("simulationMethod"), scene_has_dynamic_solids(cfg), dynamic_solids, iisph,
+                      iisph_bodies)
+    h, grid_num, m_V0, _ = scene_geometry(cfg)
+    arrays, object_collection, _, counts = assemble_particles(cfg, 3, 2 * cfg.get_cfg("particleRadius"))
     object_ids, object_sizes = np.unique(arrays["object_id"], return_counts=True)
-    ds = np.array(cfg.get_cfg("domainEnd"), dtype=np.float64) - np.array(cfg.get_cfg("domainStart"))
-    gx = int(np.ceil(ds / h).astype(int)[0])
-    lay = layer_of(arrays["x"], h)
-    hist = np.bincount(lay, minlength=gx)[:gx]
-    send_layers = SEND_LAYERS_BODIES if dynamic_solids else SEND_LAYERS
-    ghost_layers = GHOST_LAYERS_BODIES if dynamic_solids else GHOST_LAYERS
-    if dynamic_solids and cfg.get_cfg("simulationMethod") == 4:
-        raise NotImplementedError(DYNAMIC_SOLIDS_WCSPH_ONLY)
+    gx = int(grid_num[0])
+    hist = np.bincount(layer_of(arrays["x"], h), minlength=gx)[:gx]
     if slabs is None:
-        slabs = plan_slabs(hist, world, min_width=send_layers + 1)
+        slabs = plan_slabs(hist, world, min_width=mode.send_layers + 1)
     fluid = arrays["material"] == 1
-    if not dynamic_solids and bool((~fluid & (arrays["is_dynamic"] != 0)).any()):
+    if not mode.bodies and bool((~fluid & (arrays["is_dynamic"] != 0)).any()):
         raise NotImplementedError(STATIC_SOLIDS_ONLY)
     n_solid = int((~fluid).sum())
-    bodies = None
+    table, rest_cms = [], []
     if n_solid:
         arrays["solid_id"] = solid_ids(arrays)
-        arrays["m_V"] = startup_boundary_volumes(cfg, arrays, device)
-    if dynamic_solids:
-        table = dynamic_bodies(cfg, arrays) if n_solid else []
-        bodies = [t + (cm,) for t, cm in zip(table, startup_rest_cms(cfg, arrays, table, device))] if table else []
+        if mode.bodies:
+            table = dynamic_bodies(cfg, arrays)
+        arrays["m_V"], rest_cms = startup_state(cfg, arrays, table, device)
+    bodies = [t + (cm,) for t, cm in zip(table, rest_cms)] if mode.bodies else None
     lo, hi = slabs[rank]
     mine, n_mine = select_owned(arrays, h, lo, hi)
     # one decision for the whole scene (a rank may start empty), the single engine's: all FLUID particles share m
     # and m_V (solids do not count)?
-    m_V0 = np.float32(0.8 * (2 * radius) ** 3)
     m_fluid = arrays["density"][fluid].astype(np.float32) * m_V0
     uniform = bool(m_fluid.size and (m_fluid == m_fluid[0]).all())
     hint = (uniform, float(m_fluid[0]) if m_fluid.size else 0.0, float(m_V0))
     # the fullest layer bounds every layer the front may reach later: SEND_LAYERS of them per side and direction
-    halo_cap = int(send_layers * int(hist.max()) * capacity_factor) + 1024
-    ghost_est = 2 * ghost_layers * int(hist.max())
+    halo_cap = int(mode.send_layers * int(hist.max()) * capacity_factor) + 1024
+    ghost_est = 2 * mode.ghost_layers * int(hist.max())
     n_cap = int((n_mine + ghost_est) * capacity_factor) + 4 * halo_cap + 1024  # live + trash + 2 receive regions
-    sim = ShardedSimulation(cfg, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, hint, group=group,
+    sim = ShardedSimulation(cfg, mode, mine, n_mine, slabs, rank, world, device, n_cap, halo_cap, hint, group=group,
                             rebalance_every=rebalance_every, transport=transport, n_fluid=int(fluid.sum()),
-                            n_solid=n_solid, bodies=bodies, iisph_bodies=iisph_bodies)
+                            n_solid=n_solid, bodies=bodies)
     sim.object_collection = object_collection  # the meshes of the OBJ export (restPosition, restCenterOfMass)
     sim.object_counts = {int(o): int(k) for o, k in zip(object_ids, object_sizes)}
     return sim, counts["total"]

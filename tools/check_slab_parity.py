@@ -161,7 +161,7 @@ def main():
     dynamic = a.dynamic_body or a.dynamic_block
     if dynamic and not a.scene:
         sc = add_dynamic_solids(sc, c, d, world, a.dynamic_body, a.dynamic_block, a.body_vy)
-    if a.scene and any(b.get("isDynamic") for b in sc.get("RigidBodies", []) + sc.get("RigidBlocks", [])):
+    if a.scene and slab.scene_has_dynamic_solids(SimConfig(sc)):
         dynamic = True
     if not a.scene and not a.collide:
         sc["FluidBlocks"][0]["velocity"] = [a.vx, 0.0, 0.0]
@@ -207,8 +207,8 @@ def main():
     elif a.iisph:
         for _ in range(a.steps):  # one step per call: the sweep counts of every step
             sim.step(1)
-            trace.append((sim.last_iterations, sim.last_avg_err.hex()) + ((body_trace(),) if dynamic else ()))
-    elif dynamic:
+            trace.append((sim.last_iterations, sim.last_avg_err.hex()) + ((body_trace(),) if sim.mode.bodies else ()))
+    elif sim.mode.bodies:
         for _ in range(a.steps):  # one step per call: the body states of every step
             sim.step(1)
             trace.append(body_trace())
@@ -226,7 +226,7 @@ def main():
         meta["x0_ghost_right"] = x0[last["own_end"]:last["n_live"]].tolist()
         meta["x0_owned"] = x0[last["own_begin"]:last["own_end"]].tolist()
         meta["transport"] = sim.transport_stats()
-    if dynamic:
+    if sim.mode.bodies:
         meta["transport"] = sim.transport_stats()
         meta["halo_cap"] = sim.halo_cap
         meta["body_particles"] = sum(b1 - b0 for _, b0, b1, _cm in sim.bodies)
@@ -252,7 +252,7 @@ def main():
         else:
             s.step(a.steps)
         bodies = None
-        if dynamic:
+        if sim.mode.bodies:
             bodies = {oid: sim.body_state(b) for b, (oid, *_rest) in enumerate(sim.bodies)}
         cmp_ = slab.compare_with_single(gathered, ps, d, bodies=bodies)
         lo_, hi_ = (torch.tensor(sc["Configuration"][k], dtype=torch.float32) for k in ("domainStart", "domainEnd"))
@@ -290,7 +290,7 @@ def main():
                         transport_bytes=[m["transport"][1] for m in metas])
             if a.iisph:
                 cmp_.update(avg_err_sharded=[float.fromhex(t[1]) for t in metas[0]["trace"]], avg_err_single=single_errs)
-        if dynamic:
+        if sim.mode.bodies:
             same_on_ranks = all(json.dumps(m["trace"]) == json.dumps(metas[0]["trace"]) for m in metas)
             g_y, t = float(sc["Configuration"]["gravitation"][1]), a.steps * float(sc["Configuration"]["timeStepSize"])
             X, V, X0, OID, MV, FL = gathered
