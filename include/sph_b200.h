@@ -235,6 +235,45 @@ int sph_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream);
  * op 4 replaces it with the final one. */
 int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream);
 
+/* ---- PCISPH (predictive-corrective incompressible SPH, simulationMethod 1; the legacy engine's pci_* methods) ----
+ * These calls implement the 3-D formulation DESIGN.md section 11 states (its deviations from the legacy 2-D code are
+ * listed there).  sph_set_pcisph(1) puts a context in PCISPH mode: the density pass has DFSPH semantics (no clamp, no
+ * EOS), and the WCSPH, DFSPH and IISPH calls (sph_step, sph_dfsph_*, sph_iisph_*) and every sph_shard_configure* call
+ * refuse the context: PCISPH is single-GPU, and sph_set_pcisph(1) is refused on a sharded context.  sph_set_dfsph,
+ * sph_set_iisph(1) or sph_set_pcisph(0) leave the mode (sph_set_pcisph(0) on a context that is not in PCISPH mode
+ * changes nothing).  The PCISPH calls refuse a context that is not in PCISPH mode.  One op per method name:
+ *   0 compute_densities (also builds the neighbour lists)
+ *   1 pci_compute_deltas (a^np = gravity + viscosity; p = 0, a^p = 0)
+ *   2 pci_pos_vel_prediction (v* = v + dt (a^np + a^p), x* = x + dt v*; solids stay at x^t)
+ *   3 pci_update_pressure (arg = delta; out_dev = zero-initialised int32 that receives the max of the sweep's error
+ *     max(rho* - rho0, 0) as the bits of a float)
+ *   4 pci_update_pressure_force (a^p at x*)
+ *   5 compute_pressure_forces (the same a^p + reactions on dynamic solids)   6 pci_update_time_step */
+int sph_set_pcisph(SphCtx *ctx, int32_t enable);
+int sph_pcisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream);
+/* The prediction-correction loop (ops 2-4 per sweep)
+ *     it = 0;  do { sweep();  it += 1 } while (!((max_err < eta rho0 and it >= min_iterations) or it >= max_iterations))
+ * with the loop condition evaluated on the device after every sweep (batches of sweeps as in sph_dfsph_solve; the
+ * first batch is first_batch sweeps).  SYNCHRONOUS: returns it and the last max error (host pointers, may be NULL). */
+int sph_pcisph_solve(SphCtx *ctx, float delta, double eta, int32_t min_iterations, int32_t max_iterations,
+                     int32_t first_batch, int32_t *iterations_out, double *max_err_out, void *stream);
+/* nsteps whole PCISPH SPHBase.step()s: neighbour build, moving boundary volumes, ops 0-1, the loop of sph_pcisph_solve,
+ * ops 5-6, solve_rigid_body, enforce_boundary_3D(fluid) -- every kernel launched from this one call. */
+typedef struct SphPcisphStep {
+    float delta;            /* pressure per unit of density error (pci_scaling_factor; fp64 on the host, rounded) */
+    double eta;             /* the loop may stop once the max density error < eta rho0 (0.01) */
+    int32_t min_iterations; /* 3 */
+    int32_t max_iterations; /* 1000 */
+    int32_t first_batch;    /* in: sweeps launched before the first wait; out: sweeps the last step ran */
+    int32_t iterations;     /* out: sweeps of the last step's loop */
+    double max_err;         /* out: the last sweep's max density error (kg/m^3) */
+} SphPcisphStep;
+int sph_pcisph_step(SphCtx *ctx, int32_t nsteps, SphPcisphStep *io, void *stream);
+/* Per-step scratch of the last PCISPH kernels, in the current (sorted) order of sph_unpack: the predicted density
+ * rho* [n], the pressure p [n] and the pressure acceleration a^p [n][3] (device pointers, each may be NULL; 0 for
+ * solids). */
+int sph_pcisph_read(SphCtx *ctx, float *rho_star, float *p, float *ap, void *stream);
+
 /* ---- x-slab sharding across the GPUs of one node (new; the reference is single-device) -------
  * One process per GPU.  Each rank owns the cell layers [x_lo, x_hi) of the x axis (x-major flattening,
  * particle_system.py:292-294: after the sort every layer is ONE contiguous index range) and keeps

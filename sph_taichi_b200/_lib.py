@@ -29,6 +29,7 @@ ABI_SYMBOLS = [
     "sph_shard_step", "sph_halo_exchange", "sph_shard_info", "sph_shard_profile_step", "sph_shard_dfsph_step",
     "sph_shard_transport_stats", "sph_shard_configure_bodies", "sph_shard_dump", "sph_set_iisph", "sph_iisph_op",
     "sph_iisph_solve", "sph_iisph_step", "sph_iisph_read", "sph_shard_iisph_step", "sph_shard_configure_iisph_bodies",
+    "sph_set_pcisph", "sph_pcisph_op", "sph_pcisph_solve", "sph_pcisph_step", "sph_pcisph_read",
 ]
 
 
@@ -95,6 +96,11 @@ class SphDfsphStep(C.Structure):
 class SphIisphStep(C.Structure):
     _fields_ = [("max_iterations", C.c_int32), ("omega", C.c_float), ("eta", C.c_double), ("n_fluid", C.c_int64),
                 ("first_batch", C.c_int32), ("iterations", C.c_int32), ("avg_err", C.c_double)]
+
+
+class SphPcisphStep(C.Structure):
+    _fields_ = [("delta", C.c_float), ("eta", C.c_double), ("min_iterations", C.c_int32), ("max_iterations", C.c_int32),
+                ("first_batch", C.c_int32), ("iterations", C.c_int32), ("max_err", C.c_double)]
 
 
 _lib = None
@@ -176,6 +182,12 @@ def load():
         "sph_iisph_step": (C.c_int, [vp, i32, C.POINTER(SphIisphStep), vp]),
         "sph_iisph_read": (C.c_int, [vp, vp, vp, vp, vp]),
         "sph_shard_iisph_step": (C.c_int, [vp, i32, C.POINTER(SphIisphStep), vp]),
+        "sph_set_pcisph": (C.c_int, [vp, i32]),
+        "sph_pcisph_op": (C.c_int, [vp, i32, C.c_float, vp, vp]),
+        "sph_pcisph_solve": (C.c_int, [vp, C.c_float, C.c_double, i32, i32, i32, C.POINTER(i32), C.POINTER(C.c_double),
+                                       vp]),
+        "sph_pcisph_step": (C.c_int, [vp, i32, C.POINTER(SphPcisphStep), vp]),
+        "sph_pcisph_read": (C.c_int, [vp, vp, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "sph_iisph.cuh"
+#include "sph_pcisph.cuh"
 
 namespace {
 
@@ -48,9 +49,16 @@ const char *const kShardBodiesFixed =
     "the body table of a context configured by sph_shard_configure_bodies is fixed: configure a new context";
 const char *const kNoDfsph = "sph_set_dfsph(1) was not called";
 const char *const kNoIisph = "sph_set_iisph(1) was not called";
+const char *const kPcisphContext =
+    "this context is in PCISPH mode (sph_set_pcisph): it steps with sph_pcisph_op / sph_pcisph_solve / sph_pcisph_step";
+// the PCISPH calls launch over all records and exchange nothing: PCISPH is single-GPU
+const char *const kPcisphSingleGpu =
+    "PCISPH (sph_set_pcisph) is single-GPU: x-slab sharding runs WCSPH, DFSPH and IISPH contexts";
+const char *const kNoPcisph = "sph_set_pcisph(1) was not called";
 const char *const kWorldChanged = "the transport's world size changed after sph_shard_configure: configure again";
-// device copy P.dfsph, set for IISPH too: the two Jacobi solvers share the density pass (no clamp, no EOS)
-enum class Solver { WCSPH, DFSPH, IISPH };
+// device copy P.dfsph, set for IISPH and PCISPH too: the three list-based solvers share the density pass (no clamp,
+// no EOS)
+enum class Solver { WCSPH, DFSPH, IISPH, PCISPH };
 // device copy P.slab_on; Static: sph_shard_configure, Bodies: sph_shard_configure_bodies / _iisph_bodies
 enum class ShardMode { Off, Static, Bodies };
 
@@ -253,13 +261,16 @@ struct Need {
 
 // The mode checks of every entry point, in this order: configured, the entry point's bare argument checks (args_ok),
 // solver, not sharded, not a body context, begun, world size unchanged, then the neighbour structure; returns the first
-// refusal or SPH_OK.  Other solvers' entry points refuse an IISPH context with one message per kind (sharded or not).
+// refusal or SPH_OK.  Other solvers' entry points refuse an IISPH context with one message per kind (sharded or not),
+// and a PCISPH context (never sharded) with one message.
 int require(SphCtx *c, const Need &n, bool args_ok = true) {
     if (!c) return SPH_E_ARG;
     if (n.configured && c->shard == ShardMode::Off) return fail(c, SPH_E_ARG, "sph_shard_configure was not called");
     if (!args_ok) return SPH_E_ARG;
     if (n.other_solver && c->solver != n.solver)
-        return fail(c, SPH_E_ARG, c->solver == Solver::IISPH ? (n.configured ? kIisphShardStep : kIisphContext) : n.other_solver);
+        return fail(c, SPH_E_ARG, c->solver == Solver::IISPH    ? (n.configured ? kIisphShardStep : kIisphContext)
+                                  : c->solver == Solver::PCISPH ? kPcisphContext
+                                                                : n.other_solver);
     if (n.if_sharded && c->shard != ShardMode::Off) return fail(c, SPH_E_ARG, n.if_sharded);
     if (n.if_bodies && c->shard == ShardMode::Bodies) return fail(c, SPH_E_ARG, n.if_bodies);
     if (n.begun && !c->shard_begun) return fail(c, SPH_E_ARG, "sph_shard_begin was not called");
@@ -1178,6 +1189,7 @@ int check_slab_args(SphCtx *ctx, bool bodies, int32_t x_lo, int32_t x_hi, int32_
 int shard_configure_bodies(SphCtx *ctx, bool iisph, int32_t x_lo, int32_t x_hi, int32_t ghost_layers,
                            int64_t halo_capacity, int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
     if (!ctx || n_bodies < 0 || (n_bodies > 0 && !bodies)) return SPH_E_ARG;
+    if (ctx->solver == Solver::PCISPH) return fail(ctx, SPH_E_ARG, kPcisphSingleGpu);
     if ((ctx->solver == Solver::IISPH) != iisph)
         return fail(ctx, SPH_E_ARG, iisph ? kShardIisphBodiesContext : kShardBodiesIisph);
     if (int rc = check_slab_args(ctx, true, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every,
@@ -1229,6 +1241,7 @@ extern "C" {
 int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                         int32_t rebalance_every) {
     if (!ctx) return SPH_E_ARG;
+    if (ctx->solver == Solver::PCISPH) return fail(ctx, SPH_E_ARG, kPcisphSingleGpu);
     // Static solids travel in the records like fluid particles and never change; dynamic solids need moving boundary
     // volumes one ghost layer deeper, reactions across a cut and a per-body reduction across ranks: the opt-in
     // sph_shard_configure_bodies.
@@ -1449,6 +1462,13 @@ int sph_set_iisph(SphCtx *ctx, int32_t enable) {
     return SPH_OK;
 }
 
+int sph_set_pcisph(SphCtx *ctx, int32_t enable) {
+    if (int rc = require(ctx, Need().unsharded(enable ? kPcisphSingleGpu : nullptr))) return rc;
+    if (!enable && ctx->solver != Solver::PCISPH) return SPH_OK;  // not in PCISPH mode: the context stays as it is
+    set_solver(ctx, enable ? Solver::PCISPH : Solver::WCSPH);
+    return SPH_OK;
+}
+
 int sph_dfsph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
     if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph))) return rc;
     const DevParams &P = ctx->P;
@@ -1624,6 +1644,48 @@ int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double et
     });
 }
 
+// The prediction-correction loop of PCISPH as a device_loop: per sweep k_pcisph_predict, k_pcisph_update_pressure (error
+// max fused), k_pcisph_pressure_force<false> and k_pcisph_check.  Single-GPU: over all n records.
+int pcisph_solve_loop(SphCtx *ctx, float delta, double eta, int32_t min_iterations, int32_t max_iterations,
+                      int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t *kernels) {
+    const DevParams &P = ctx->P;
+    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
+    const double threshold = eta * (double)P.rho0;
+    return device_loop(ctx, first_batch, 4, h, st, kernels, [&](DfsphCtrl *ctrl) {
+        k_pcisph_predict<<<b256, 256, 0, st>>>(P, ctx->S, ctrl);
+        k_pcisph_update_pressure<<<b128, 128, 0, st>>>(P, ctx->S, delta, &ctrl->err_max, ctrl);
+        k_pcisph_pressure_force<false><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+        k_pcisph_check<<<1, 1, 0, st>>>(ctrl, threshold, min_iterations, max_iterations);
+        return SPH_OK;
+    });
+}
+
+// The PCISPH substep (DESIGN section 11): densities (+ lists) -> pci_compute_deltas (non-pressure forces without
+// cohesion, then p = 0, a^p = 0) -> the prediction-correction loop -> compute_pressure_forces (the last sweep's a^p
+// again, now with the reactions on dynamic solids: once per step, after the loop) -> pci_update_time_step.  io:
+// constants in, counts out.
+int launch_pcisph_substep(SphCtx *c, cudaStream_t st, SphPcisphStep *io, int64_t *kernels) {
+    const DevParams &P = c->P;
+    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
+    launch_pair_density(c, st, kernels);
+    c->list_valid = true;
+    DevParams Pn = P;
+    Pn.sigma = 0.0f;  // PCISPH's non-pressure forces are gravity + viscosity: the cohesion term is an exact zero
+    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, c->S);
+    k_pcisph_init<<<b256, 256, 0, st>>>(P, c->S);
+    *kernels += 2;
+    DfsphCtrl h{};
+    int rc = pcisph_solve_loop(c, io->delta, io->eta, io->min_iterations, io->max_iterations, io->first_batch, &h, st,
+                               kernels);
+    if (rc) return rc;
+    io->iterations = h.iterations; io->max_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
+    k_pcisph_pressure_force<true><<<b128, 128, 0, st>>>(P, c->S, nullptr);
+    k_pcisph_advect<<<b256, 256, 0, st>>>(P, c->S);
+    *kernels += 2;
+    c->built = false; c->list_valid = false;  // positions moved
+    return SPH_OK;
+}
+
 // IISPH.substep (DESIGN section 10) over the sorted records [0, n_grid): densities (+ lists) -> non-pressure forces
 // without cohesion -> predict_advection -> pressure_solve -> compute_pressure_forces (+ reactions) -> advect.  io:
 // constants in, counts out.  The exchanges run only on a sharded context: v* after predict_velocity (read by
@@ -1723,7 +1785,8 @@ int launch_dfsph_substep(SphCtx *c, cudaStream_t st, SphDfsphStep *io, int64_t n
     return SPH_OK;
 }
 
-// One single-GPU SPHBase.step() (sph_base.py:263-271) of a solver whose substep launches itself (DFSPH, IISPH):
+// One single-GPU SPHBase.step() (sph_base.py:263-271) of a solver whose substep launches itself (DFSPH, IISPH,
+// PCISPH):
 //   neighbour build -> moving boundary volumes -> substep() -> solve_rigid_body -> enforce_boundary_3D(fluid)
 template <typename Substep>
 int single_step(SphCtx *ctx, cudaStream_t st, Substep substep) {
@@ -1884,6 +1947,92 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) 
     if (int rc = require(ctx, Need().runs(Solver::IISPH, kNoIisph))) return rc;
     if (ctx->P.n == 0) return SPH_OK;
     k_iisph_read<<<blocks_for(ctx->P.n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S, a_ii, s, ap);
+    ctx->launches += 1;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return SPH_OK;
+}
+
+int sph_pcisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
+    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu))) return rc;
+    const DevParams &P = ctx->P;
+    if (P.n == 0) return SPH_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
+    if (op < PCISPH_COMPUTE_DENSITIES || op > PCISPH_UPDATE_TIME_STEP) return fail(ctx, SPH_E_ARG, "unknown PCISPH op");
+    if (!ctx->built) return fail(ctx, SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first");
+    if (op != PCISPH_COMPUTE_DENSITIES && op != PCISPH_UPDATE_TIME_STEP && !ctx->list_valid)
+        return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run op 0 (compute_densities) first");
+    if (op == PCISPH_UPDATE_PRESSURE && !out_dev) return SPH_E_ARG;
+    DevParams Pn = P;
+    switch (op) {
+        case PCISPH_COMPUTE_DENSITIES:
+            launch_pair_density(ctx, st, &ctx->launches);
+            ctx->list_valid = true;
+            break;
+        case PCISPH_COMPUTE_DELTAS:
+            Pn.sigma = 0.0f;  // gravity + viscosity only
+            k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, ctx->S);
+            k_pcisph_init<<<b256, 256, 0, st>>>(P, ctx->S);
+            ctx->launches += 2;
+            break;
+        case PCISPH_POS_VEL_PREDICTION:
+            k_pcisph_predict<<<b256, 256, 0, st>>>(P, ctx->S, nullptr);
+            ctx->launches += 1;
+            break;
+        case PCISPH_UPDATE_PRESSURE:
+            k_pcisph_update_pressure<<<b128, 128, 0, st>>>(P, ctx->S, arg, static_cast<int32_t *>(out_dev), nullptr);
+            ctx->launches += 1;
+            break;
+        case PCISPH_UPDATE_PRESSURE_FORCE:
+            k_pcisph_pressure_force<false><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
+            ctx->launches += 1;
+            break;
+        case PCISPH_COMPUTE_PRESSURE_FORCES:
+            k_pcisph_pressure_force<true><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
+            ctx->launches += 1;
+            break;
+        case PCISPH_UPDATE_TIME_STEP:
+            k_pcisph_advect<<<b256, 256, 0, st>>>(P, ctx->S);
+            ctx->launches += 1;
+            ctx->built = false; ctx->list_valid = false;
+            break;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    return SPH_OK;
+}
+
+int sph_pcisph_solve(SphCtx *ctx, float delta, double eta, int32_t min_iterations, int32_t max_iterations,
+                     int32_t first_batch, int32_t *iterations_out, double *max_err_out, void *stream) {
+    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu).fresh_lists(),
+                         max_iterations >= 1))
+        return rc;
+    DfsphCtrl h{};
+    int rc = pcisph_solve_loop(ctx, delta, eta, min_iterations, max_iterations, first_batch, &h,
+                               static_cast<cudaStream_t>(stream), &ctx->launches);
+    if (rc) return rc;
+    if (iterations_out) *iterations_out = h.iterations;
+    if (max_err_out) *max_err_out = h.last_avg;
+    return SPH_OK;
+}
+
+int sph_pcisph_step(SphCtx *ctx, int32_t nsteps, SphPcisphStep *io, void *stream) {
+    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu),
+                         io && nsteps >= 0 && io->max_iterations >= 1))
+        return rc;
+    if (ctx->P.n == 0) return SPH_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int s = 0; s < nsteps; ++s) {
+        int rc = single_step(ctx, st, [&] { return launch_pcisph_substep(ctx, st, io, &ctx->launches); });
+        if (rc) return rc;
+    }
+    return SPH_OK;
+}
+
+int sph_pcisph_read(SphCtx *ctx, float *rho_star, float *p, float *ap, void *stream) {
+    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph))) return rc;
+    if (ctx->P.n == 0) return SPH_OK;
+    k_pcisph_read<<<blocks_for(ctx->P.n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(ctx->P, ctx->S, rho_star, p,
+                                                                                              ap);
     ctx->launches += 1;
     CUDA_TRY(ctx, cudaGetLastError());
     return SPH_OK;

@@ -32,7 +32,7 @@ struct DfsphCtrl {
     int32_t iterations;  // the reference's m_iterations(_v): sweeps that did NOT meet eta
     int32_t done;        // loop left (converged, or the iteration cap reached)
     int32_t sweeps;      // sweeps actually executed
-    int32_t pad;
+    int32_t err_max;     // PCISPH: the running max of the sweep's error, as the int bits of a non-negative float
 };
 
 // Dense walk over the neighbour list of particle i (reference visiting order), gathers batched by

@@ -235,6 +235,32 @@ class Engine:
         ptr = [None if t is None else t.data_ptr() for t in (a_ii, s, ap)]
         self._check(self.lib.sph_iisph_read(self.ctx, *ptr, self._stream()), "sph_iisph_read")
 
+    def set_pcisph(self, enable=True):
+        self._check(self.lib.sph_set_pcisph(self.ctx, int(bool(enable))), "sph_set_pcisph")
+
+    def pcisph_op(self, op, arg=0.0, out=None):
+        self._check(self.lib.sph_pcisph_op(self.ctx, int(op), float(arg), None if out is None else out.data_ptr(),
+                                           self._stream()), "sph_pcisph_op")
+
+    def pcisph_solve(self, delta, eta, min_iterations, max_iterations, first_batch):
+        """The prediction-correction loop with its condition on the device; returns (iterations, last max error).
+        Synchronous (one wait per batch of sweeps)."""
+        it, err = C.c_int32(0), C.c_double(0.0)
+        self._check(self.lib.sph_pcisph_solve(self.ctx, float(delta), float(eta), int(min_iterations),
+                                              int(max_iterations), int(first_batch), C.byref(it), C.byref(err),
+                                              self._stream()), "sph_pcisph_solve")
+        return int(it.value), float(err.value)
+
+    def pcisph_step(self, nsteps, io):
+        """`nsteps` whole PCISPH steps launched from one call; `io` is a _lib.SphPcisphStep (constants in, counts
+        out)."""
+        self._check(self.lib.sph_pcisph_step(self.ctx, int(nsteps), C.byref(io), self._stream()), "sph_pcisph_step")
+
+    def pcisph_read(self, rho_star=None, p=None, ap=None):
+        """rho* [n], p [n], a^p [n, 3] (float32 tensors on the engine's device, each may be None), sorted order."""
+        ptr = [None if t is None else t.data_ptr() for t in (rho_star, p, ap)]
+        self._check(self.lib.sph_pcisph_read(self.ctx, *ptr, self._stream()), "sph_pcisph_read")
+
     def step(self, nsteps=1):
         self._check(self.lib.sph_step(self.ctx, int(nsteps), self._stream()), "sph_step")
 

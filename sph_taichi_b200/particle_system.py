@@ -241,6 +241,9 @@ class ParticleSystem:
         if solver_type == 3:
             from .IISPH import IISPHSolver
             return IISPHSolver(self)
+        if solver_type == 1:
+            from .PCISPH import PCISPHSolver
+            return PCISPHSolver(self)
         raise NotImplementedError(f"Solver type {solver_type} has not been implemented.")
 
     def add_particles(self, object_id, new_particles_num, new_particles_positions, new_particles_velocity,

@@ -161,6 +161,17 @@ def _as_iisph(sc, dt=0.001):
     return sc
 
 
+def _as_pcisph(sc, dt=0.001):
+    sc["Configuration"]["simulationMethod"] = 1
+    sc["Configuration"]["timeStepSize"] = dt
+    return sc
+
+
+def dragon_bath_pcisph():
+    """dragon_bath's geometry with the PCISPH solver (simulationMethod 1), dt = 1e-3 (DESIGN.md section 11)."""
+    return _as_pcisph(dragon_bath())
+
+
 def dragon_bath_iisph():
     """dragon_bath's geometry with the IISPH solver (simulationMethod 3), dt = 1e-3 (DESIGN.md section 10)."""
     return _as_iisph(dragon_bath())
@@ -204,6 +215,7 @@ NAMED_SCENES = {
     "high_fluid_wcsph": high_fluid_wcsph,
     "dragon_bath_dfsph": dragon_bath_dfsph,
     "dragon_bath_iisph": dragon_bath_iisph,
+    "dragon_bath_pcisph": dragon_bath_pcisph,
     "dragon_bath_dynamic_dfsph": dragon_bath_dynamic_dfsph,
     "high_fluid_dfsph": high_fluid_dfsph,
     "armadillo_bath_dynamic_dfsph": armadillo_bath_dynamic_dfsph,
