@@ -46,6 +46,8 @@ def dfsph_step_io(dt, density0, n_fluid, first_batch_v=FIRST_BATCHES[0], first_b
 
 
 class DFSPHSolver(SPHBase):
+    _ENGINE_OP, _ENGINE_STEP = "dfsph_op", "dfsph_step"
+
     def __init__(self, particle_system):
         super().__init__(particle_system)
         self.surface_tension = 0.01
@@ -63,11 +65,6 @@ class DFSPHSolver(SPHBase):
         self._sweeps_guess = list(FIRST_BATCHES)  # first batches of the next two solves (updated every step)
         self.ps._engine.set_dfsph(True)
         self._err = torch.zeros(1, dtype=torch.float64, device=self.ps.device)
-
-    def _op(self, op, arg=0.0, out=None):
-        self.ps._push()
-        self.ps._engine.dfsph_op(op, arg, out)
-        self.ps._after_engine()
 
     # ---- kernels (DFSPH.py names) ------------------------------------------------------------
     def compute_densities(self):
@@ -173,23 +170,14 @@ class DFSPHSolver(SPHBase):
         """sph_base.py:263-271.  With device-side loops the whole step is one library call."""
         if not self.device_side_loops:
             return super().step(n)
-        ps = self.ps
-        io = dfsph_step_io(self.dt[None], self.density_0, ps.fluid_particle_num, *self._sweeps_guess,
-                           enable_divergence_solver=self.enable_divergence_solver,
-                           max_iterations_v=self.m_max_iterations_v, max_iterations=self.m_max_iterations,
-                           max_error_v=self.max_error_V, max_error=self.max_error)
-        ps._push()
-        ps._engine.dfsph_step(n, io)
-        ps._after_engine()
-        self._sweeps_guess = [int(io.first_batch_v), int(io.first_batch)]
+        io = self._solver_step(n, dfsph_step_io(
+            self.dt[None], self.density_0, self.ps.fluid_particle_num, *self._sweeps_guess,
+            enable_divergence_solver=self.enable_divergence_solver, max_iterations_v=self.m_max_iterations_v,
+            max_iterations=self.m_max_iterations, max_error_v=self.max_error_V, max_error=self.max_error))
         self.last_iterations_v, self.last_iterations = int(io.iterations_v), int(io.iterations)
         if self.verbose:
             print(f"DFSPH - iteration V: {self.last_iterations_v} Avg density err: {io.avg_err_v}")
             print(f"DFSPH - iterations: {self.last_iterations} Avg density Err: {io.avg_err:.4f}")
-        if ps.cfg.get_cfg("exportObj"):
-            for oid in ps._body_index:
-                if "restPosition" in ps.object_collection[oid]:
-                    self._update_mesh(oid)
 
     def substep(self):
         self.compute_densities()

@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import torch
 
+from .fields import ScratchField
 from .sph_base import SPHBase
 
 (OP_DENSITIES, OP_NON_PRESSURE, OP_PREDICT_ADVECTION, OP_PRESSURE_SOLVE_ITERATION, OP_PRESSURE_FORCES,
@@ -39,28 +40,9 @@ def iisph_step_io(n_fluid, first_batch=FIRST_BATCH, *, omega=OMEGA, max_iteratio
                         n_fluid=int(n_fluid), first_batch=int(first_batch))
 
 
-class _ScratchField:
-    """Read-only per-particle scratch of the last IISPH kernels (a_ii, s_i or a^p), in the public fields' order."""
-
-    def __init__(self, solver, which, width):
-        self._solver, self._which, self._width = solver, which, width
-
-    @property
-    def shape(self):
-        return (self._solver.ps.particle_max_num,)
-
-    def to_numpy(self):
-        ps = self._solver.ps
-        ps._push()
-        n = ps.particle_max_num
-        out = torch.zeros((n, 3) if self._width == 3 else (n,), dtype=torch.float32, device=ps.device)
-        args = [None, None, None]
-        args[self._which] = out
-        ps._engine.iisph_read(*args)
-        return out.cpu().numpy()
-
-
 class IISPHSolver(SPHBase):
+    _ENGINE_OP, _ENGINE_STEP = "iisph_op", "iisph_step"
+
     def __init__(self, particle_system):
         super().__init__(particle_system)
         self.surface_tension = 0.0  # IISPH.py's non-pressure forces are gravity + viscosity
@@ -75,14 +57,9 @@ class IISPHSolver(SPHBase):
         self._sweeps_guess = FIRST_BATCH
         self.ps._engine.set_iisph(True)
         self._err = torch.zeros(1, dtype=torch.float64, device=self.ps.device)
-        self.a_ii = _ScratchField(self, 0, 1)
-        self.density_deviation = _ScratchField(self, 1, 1)
-        self.pressure_accel = _ScratchField(self, 2, 3)
-
-    def _op(self, op, arg=0.0, out=None):
-        self.ps._push()
-        self.ps._engine.iisph_op(op, arg, out)
-        self.ps._after_engine()
+        self.a_ii = ScratchField(self, "iisph_read", 0, 1)
+        self.density_deviation = ScratchField(self, "iisph_read", 1, 1)
+        self.pressure_accel = ScratchField(self, "iisph_read", 2, 3)
 
     def step_io(self):
         """The ``SphIisphStep`` of ``sph_iisph_step`` from this solver's constants."""
@@ -141,16 +118,7 @@ class IISPHSolver(SPHBase):
         """sph_base.py:263-271.  With device-side loops the whole step is one library call."""
         if not self.device_side_loops:
             return super().step(n)
-        ps = self.ps
-        io = self.step_io()
-        ps._push()
-        ps._engine.iisph_step(n, io)
-        ps._after_engine()
-        self._sweeps_guess = int(io.first_batch)
+        io = self._solver_step(n, self.step_io())
         self.last_iterations, self.last_avg_density_error = int(io.iterations), float(io.avg_err)
         if self.verbose:
             print(f"IISPH - iterations: {self.last_iterations} Avg density err: {self.last_avg_density_error:.3e}")
-        if ps.cfg.get_cfg("exportObj"):
-            for oid in ps._body_index:
-                if "restPosition" in ps.object_collection[oid]:
-                    self._update_mesh(oid)

@@ -19,6 +19,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from .fields import ScratchField
 from .sph_base import SPHBase
 
 (OP_DENSITIES, OP_COMPUTE_DELTAS, OP_POS_VEL_PREDICTION, OP_UPDATE_PRESSURE, OP_UPDATE_PRESSURE_FORCE,
@@ -60,28 +61,9 @@ def pcisph_step_io(delta, first_batch=FIRST_BATCH, *, max_error=MAX_ERROR, min_i
                          max_iterations=int(max_iterations), first_batch=int(first_batch))
 
 
-class _ScratchField:
-    """Read-only per-particle scratch of the last PCISPH kernels (rho*, p or a^p), in the public fields' order."""
-
-    def __init__(self, solver, which, width):
-        self._solver, self._which, self._width = solver, which, width
-
-    @property
-    def shape(self):
-        return (self._solver.ps.particle_max_num,)
-
-    def to_numpy(self):
-        ps = self._solver.ps
-        ps._push()
-        n = ps.particle_max_num
-        out = torch.zeros((n, 3) if self._width == 3 else (n,), dtype=torch.float32, device=ps.device)
-        args = [None, None, None]
-        args[self._which] = out
-        ps._engine.pcisph_read(*args)
-        return out.cpu().numpy()
-
-
 class PCISPHSolver(SPHBase):
+    _ENGINE_OP, _ENGINE_STEP = "pcisph_op", "pcisph_step"
+
     def __init__(self, particle_system):
         super().__init__(particle_system)
         self.surface_tension = 0.0  # the non-pressure forces are gravity + viscosity
@@ -97,14 +79,9 @@ class PCISPHSolver(SPHBase):
         self._sweeps_guess = FIRST_BATCH
         self.ps._engine.set_pcisph(True)
         self._err = torch.zeros(1, dtype=torch.int32, device=self.ps.device)
-        self.predicted_density = _ScratchField(self, 0, 1)
-        self.pressure_accel = _ScratchField(self, 2, 3)
+        self.predicted_density = ScratchField(self, "pcisph_read", 0, 1)
+        self.pressure_accel = ScratchField(self, "pcisph_read", 2, 3)
         self.pci_scaling_factor()
-
-    def _op(self, op, arg=0.0, out=None):
-        self.ps._push()
-        self.ps._engine.pcisph_op(op, arg, out)
-        self.ps._after_engine()
 
     def step_io(self):
         """The ``SphPcisphStep`` of ``sph_pcisph_step`` from this solver's constants."""
@@ -183,17 +160,8 @@ class PCISPHSolver(SPHBase):
         """sph_base.py:263-271.  With device-side loops the whole step is one library call."""
         if not self.device_side_loops:
             return super().step(n)
-        ps = self.ps
         self.pci_scaling_factor()
-        io = self.step_io()
-        ps._push()
-        ps._engine.pcisph_step(n, io)
-        ps._after_engine()
-        self._sweeps_guess = int(io.first_batch)
+        io = self._solver_step(n, self.step_io())
         self.last_iterations, self.last_max_density_error = int(io.iterations), float(io.max_err)
         if self.verbose:
             print(f"PCISPH - iterations: {self.last_iterations} Max density err: {self.last_max_density_error:.3e}")
-        if ps.cfg.get_cfg("exportObj"):
-            for oid in ps._body_index:
-                if "restPosition" in ps.object_collection[oid]:
-                    self._update_mesh(oid)

@@ -1469,47 +1469,6 @@ int sph_set_pcisph(SphCtx *ctx, int32_t enable) {
     return SPH_OK;
 }
 
-int sph_dfsph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
-    if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph))) return rc;
-    const DevParams &P = ctx->P;
-    if (P.n == 0) return SPH_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
-    if (op >= DFSPH_COMPUTE_DENSITIES && op <= DFSPH_NON_PRESSURE_FORCES && op != DFSPH_DENSITY_ERROR &&
-        op != DFSPH_MULTIPLY_FACTOR) {
-        if (!ctx->built)
-            return fail(ctx, SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first");
-        if (op != DFSPH_COMPUTE_DENSITIES && !ctx->list_valid)
-            return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run op 0 (compute_densities) first");
-    }
-    switch (op) {
-        case DFSPH_COMPUTE_DENSITIES:
-            launch_pair_density(ctx, st, &ctx->launches);
-            ctx->list_valid = true;
-            break;
-        case DFSPH_COMPUTE_FACTOR: k_dfsph_factor<<<b128, 128, 0, st>>>(P, ctx->S); break;
-        case DFSPH_DENSITY_CHANGE: k_dfsph_density_change<0><<<b128, 128, 0, st>>>(P, ctx->S); break;
-        case DFSPH_DENSITY_ADV: k_dfsph_density_change<1><<<b128, 128, 0, st>>>(P, ctx->S); break;
-        case DFSPH_DENSITY_ERROR:
-            if (!out_dev) return SPH_E_ARG;
-            k_dfsph_density_error<<<b256, 256, 0, st>>>(P, ctx->S, arg, static_cast<double *>(out_dev));
-            break;
-        case DFSPH_MULTIPLY_FACTOR: k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, ctx->S, arg); break;
-        case DFSPH_DIVERGENCE_ITERATION: k_dfsph_iteration<0><<<b128, 128, 0, st>>>(P, ctx->S, nullptr); break;
-        case DFSPH_PRESSURE_ITERATION: k_dfsph_iteration<1><<<b128, 128, 0, st>>>(P, ctx->S, nullptr); break;
-        case DFSPH_NON_PRESSURE_FORCES: k_dfsph_non_pressure<<<b128, 128, 0, st>>>(P, ctx->S); break;
-        case DFSPH_PREDICT_VELOCITY: k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, ctx->S); break;
-        case DFSPH_ADVECT:
-            k_dfsph_advect<<<b256, 256, 0, st>>>(P, ctx->S);
-            ctx->built = false; ctx->list_valid = false;
-            break;
-        default: return fail(ctx, SPH_E_ARG, "unknown DFSPH op");
-    }
-    if (op != DFSPH_COMPUTE_DENSITIES) ctx->launches += 1;
-    CUDA_TRY(ctx, cudaGetLastError());
-    return SPH_OK;
-}
-
 }  // extern "C"
 namespace {
 
@@ -1567,14 +1526,102 @@ int shard_dfsph_exchange(SphCtx *c, cudaStream_t st, int what, DfsphCtrl *ctrl, 
     return SPH_OK;
 }
 
+// ---- solver stages ------------------------------------------------------------------------
+// One launcher per stage of DFSPH, IISPH and PCISPH, shared by their ops, substeps and device-loop sweeps: it launches
+// the stage over the sorted records [0, n_grid) (PCISPH: all P.n), counts its kernels into *kernels and applies the
+// stage's change to the neighbour state.  Launchers never exchange: on a sharded context the substeps and sweeps issue
+// the halo messages between them.  ctrl (may be NULL): a device loop's control block.  reactions: the pressure forces
+// of compute_pressure_forces, which also scatter the reactions onto dynamic solids.
+void solver_densities(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    launch_pair_density(c, st, kernels, /*split_mode=*/0, n_grid);
+    c->list_valid = true;
+}
+// cohesion = false (IISPH, PCISPH): gravity + viscosity only; sigma = 0 makes the cohesion term an exact zero
+void non_pressure_forces(SphCtx *c, cudaStream_t st, int64_t n_grid, bool cohesion, int64_t *kernels) {
+    DevParams P = c->P;
+    if (!cohesion) P.sigma = 0.0f;
+    k_dfsph_non_pressure<<<blocks_for(n_grid, 128), 128, 0, st>>>(P, c->S);
+    *kernels += 1;
+}
+void predict_velocity(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    k_dfsph_predict_velocity<<<blocks_for(n_grid, 256), 256, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+}
+void dfsph_factor(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    k_dfsph_factor<<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+}
+// mode 0: density change (divergence solve), 1: density_adv (pressure solve); the same modes for dfsph_iteration
+void dfsph_density_change(SphCtx *c, cudaStream_t st, int64_t n_grid, int mode, int64_t *kernels) {
+    if (mode == 0) k_dfsph_density_change<0><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S);
+    else k_dfsph_density_change<1><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+}
+void dfsph_multiply_factor(SphCtx *c, cudaStream_t st, int64_t n_grid, float time_step, int64_t *kernels) {
+    k_dfsph_multiply_factor<<<blocks_for(n_grid, 256), 256, 0, st>>>(c->P, c->S, time_step);
+    *kernels += 1;
+}
+void dfsph_iteration(SphCtx *c, cudaStream_t st, int64_t n_grid, int mode, DfsphCtrl *ctrl, int64_t *kernels) {
+    if (mode == 0) k_dfsph_iteration<0><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+    else k_dfsph_iteration<1><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+    *kernels += 1;
+}
+void dfsph_advect(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    k_dfsph_advect<<<blocks_for(n_grid, 256), 256, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+    c->built = false; c->list_valid = false;  // positions moved
+}
+void iisph_predict(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    k_iisph_predict<<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+}
+void iisph_pressure_accel(SphCtx *c, cudaStream_t st, int64_t n_grid, bool reactions, DfsphCtrl *ctrl,
+                          int64_t *kernels) {
+    if (reactions) k_iisph_pressure_accel<true><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+    else k_iisph_pressure_accel<false><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+    *kernels += 1;
+}
+void iisph_pressure_update(SphCtx *c, cudaStream_t st, int64_t n_grid, float omega, double *err, DfsphCtrl *ctrl,
+                           int64_t *kernels) {
+    k_iisph_pressure_update<<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, omega, err, ctrl);
+    *kernels += 1;
+}
+void iisph_advect(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    k_iisph_advect<<<blocks_for(n_grid, 256), 256, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+    c->built = false; c->list_valid = false;  // positions moved
+}
+void pcisph_init(SphCtx *c, cudaStream_t st, int64_t *kernels) {
+    k_pcisph_init<<<blocks_for(c->P.n, 256), 256, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+}
+void pcisph_predict(SphCtx *c, cudaStream_t st, DfsphCtrl *ctrl, int64_t *kernels) {
+    k_pcisph_predict<<<blocks_for(c->P.n, 256), 256, 0, st>>>(c->P, c->S, ctrl);
+    *kernels += 1;
+}
+void pcisph_update_pressure(SphCtx *c, cudaStream_t st, float delta, int32_t *err_max, DfsphCtrl *ctrl,
+                            int64_t *kernels) {
+    k_pcisph_update_pressure<<<blocks_for(c->P.n, 128), 128, 0, st>>>(c->P, c->S, delta, err_max, ctrl);
+    *kernels += 1;
+}
+void pcisph_pressure_force(SphCtx *c, cudaStream_t st, bool reactions, DfsphCtrl *ctrl, int64_t *kernels) {
+    if (reactions) k_pcisph_pressure_force<true><<<blocks_for(c->P.n, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+    else k_pcisph_pressure_force<false><<<blocks_for(c->P.n, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+    *kernels += 1;
+}
+void pcisph_advect(SphCtx *c, cudaStream_t st, int64_t *kernels) {
+    k_pcisph_advect<<<blocks_for(c->P.n, 256), 256, 0, st>>>(c->P, c->S);
+    *kernels += 1;
+    c->built = false; c->list_valid = false;  // positions moved
+}
+
 // A Jacobi loop with its loop condition on the device: sweeps are launched in batches (the first as long as the
 // caller expects the loop to run -- the previous step's count is a good guess), every sweep ends with a check kernel
 // that updates the DfsphCtrl in the workspace scratch block, sweeps behind the converged one return at once, and the
-// host reads the control block once per batch.  sweep(ctrl) launches one sweep, check included, and returns 0 or an
-// SPH_E_* code; each sweep counts `sweep_kernels` kernels (plus whatever it counts itself).
+// host reads the control block once per batch.  sweep(ctrl) launches one sweep, check included, counts its kernels
+// and returns 0 or an SPH_E_* code.
 template <typename Sweep>
-int device_loop(SphCtx *ctx, int32_t first_batch, int sweep_kernels, DfsphCtrl *h, cudaStream_t st, int64_t *kernels,
-                Sweep sweep) {
+int device_loop(SphCtx *ctx, int32_t first_batch, DfsphCtrl *h, cudaStream_t st, Sweep sweep) {
     DfsphCtrl *ctrl = reinterpret_cast<DfsphCtrl *>(ctx->ws + ctx->L.off_scratch);
     *h = DfsphCtrl{};
     CUDA_TRY(ctx, cudaMemsetAsync(ctrl, 0, sizeof(DfsphCtrl), st));
@@ -1583,7 +1630,6 @@ int device_loop(SphCtx *ctx, int32_t first_batch, int sweep_kernels, DfsphCtrl *
     while (!h->done) {
         for (int s = 0; s < batch; ++s)
             if (int rc = sweep(ctrl)) return rc;
-        *kernels += sweep_kernels * (int64_t)batch;
         CUDA_TRY(ctx, cudaGetLastError());
         CUDA_TRY(ctx, cudaMemcpyAsync(h, ctrl, sizeof(DfsphCtrl), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(ctx, cudaStreamSynchronize(st));
@@ -1601,9 +1647,8 @@ int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, 
                      int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
     const DevParams &P = ctx->P;
     const int b128 = blocks_for(n_grid, 128);
-    return device_loop(ctx, first_batch, 3, h, st, kernels, [&](DfsphCtrl *ctrl) {
-        if (mode == 0) k_dfsph_iteration<0><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
-        else k_dfsph_iteration<1><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+    return device_loop(ctx, first_batch, h, st, [&](DfsphCtrl *ctrl) {
+        dfsph_iteration(ctx, st, n_grid, mode, ctrl, kernels);
         int rc = shard_dfsph_exchange(ctx, st, DX_VELD, ctrl, false, kernels);
         if (rc) return rc;
         if (mode == 0) k_dfsph_density_change_err<0><<<b128, 128, 0, st>>>(P, ctx->S, offset, ctrl);
@@ -1615,6 +1660,7 @@ int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, 
                                                   max_iterations);
         else
             k_dfsph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
+        *kernels += 2;  // the density change and the check
         return SPH_OK;
     });
 }
@@ -1626,20 +1672,19 @@ int dfsph_solve_loop(SphCtx *ctx, int mode, int32_t max_iterations, double eta, 
 // for k_iisph_check_ranked; n_fluid is then the global fluid count.
 int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double eta, int64_t n_fluid, int32_t first_batch,
                      DfsphCtrl *h, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
-    const DevParams &P = ctx->P;
-    const int b128 = blocks_for(n_grid, 128);
-    return device_loop(ctx, first_batch, 3, h, st, kernels, [&](DfsphCtrl *ctrl) {
-        k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+    return device_loop(ctx, first_batch, h, st, [&](DfsphCtrl *ctrl) {
+        iisph_pressure_accel(ctx, st, n_grid, /*reactions=*/false, ctrl, kernels);
         int rc = shard_dfsph_exchange(ctx, st, DX_ACC, ctrl, false, kernels);
         if (rc) return rc;
-        k_iisph_pressure_update<<<b128, 128, 0, st>>>(P, ctx->S, omega, &ctrl->err, ctrl);
+        iisph_pressure_update(ctx, st, n_grid, omega, &ctrl->err, ctrl, kernels);
         rc = shard_dfsph_exchange(ctx, st, DX_AUX, ctrl, true, kernels);
         if (rc) return rc;
-        if (P.slab_on)
+        if (ctx->P.slab_on)
             k_iisph_check_ranked<<<1, 1, 0, st>>>(ctrl, shard_err_parts(ctx), ctx->rank, ctx->world, (double)n_fluid, eta,
                                                   max_iterations);
         else
             k_iisph_check<<<1, 1, 0, st>>>(ctrl, (double)n_fluid, eta, max_iterations);
+        *kernels += 1;
         return SPH_OK;
     });
 }
@@ -1648,14 +1693,13 @@ int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double et
 // max fused), k_pcisph_pressure_force<false> and k_pcisph_check.  Single-GPU: over all n records.
 int pcisph_solve_loop(SphCtx *ctx, float delta, double eta, int32_t min_iterations, int32_t max_iterations,
                       int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t *kernels) {
-    const DevParams &P = ctx->P;
-    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
-    const double threshold = eta * (double)P.rho0;
-    return device_loop(ctx, first_batch, 4, h, st, kernels, [&](DfsphCtrl *ctrl) {
-        k_pcisph_predict<<<b256, 256, 0, st>>>(P, ctx->S, ctrl);
-        k_pcisph_update_pressure<<<b128, 128, 0, st>>>(P, ctx->S, delta, &ctrl->err_max, ctrl);
-        k_pcisph_pressure_force<false><<<b128, 128, 0, st>>>(P, ctx->S, ctrl);
+    const double threshold = eta * (double)ctx->P.rho0;
+    return device_loop(ctx, first_batch, h, st, [&](DfsphCtrl *ctrl) {
+        pcisph_predict(ctx, st, ctrl, kernels);
+        pcisph_update_pressure(ctx, st, delta, &ctrl->err_max, ctrl, kernels);
+        pcisph_pressure_force(ctx, st, /*reactions=*/false, ctrl, kernels);
         k_pcisph_check<<<1, 1, 0, st>>>(ctrl, threshold, min_iterations, max_iterations);
+        *kernels += 1;
         return SPH_OK;
     });
 }
@@ -1665,24 +1709,16 @@ int pcisph_solve_loop(SphCtx *ctx, float delta, double eta, int32_t min_iteratio
 // again, now with the reactions on dynamic solids: once per step, after the loop) -> pci_update_time_step.  io:
 // constants in, counts out.
 int launch_pcisph_substep(SphCtx *c, cudaStream_t st, SphPcisphStep *io, int64_t *kernels) {
-    const DevParams &P = c->P;
-    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
-    launch_pair_density(c, st, kernels);
-    c->list_valid = true;
-    DevParams Pn = P;
-    Pn.sigma = 0.0f;  // PCISPH's non-pressure forces are gravity + viscosity: the cohesion term is an exact zero
-    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, c->S);
-    k_pcisph_init<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 2;
+    solver_densities(c, st, c->P.n, kernels);
+    non_pressure_forces(c, st, c->P.n, /*cohesion=*/false, kernels);
+    pcisph_init(c, st, kernels);
     DfsphCtrl h{};
     int rc = pcisph_solve_loop(c, io->delta, io->eta, io->min_iterations, io->max_iterations, io->first_batch, &h, st,
                                kernels);
     if (rc) return rc;
     io->iterations = h.iterations; io->max_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-    k_pcisph_pressure_force<true><<<b128, 128, 0, st>>>(P, c->S, nullptr);
-    k_pcisph_advect<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 2;
-    c->built = false; c->list_valid = false;  // positions moved
+    pcisph_pressure_force(c, st, /*reactions=*/true, nullptr, kernels);
+    pcisph_advect(c, st, kernels);
     return SPH_OK;
 }
 
@@ -1696,18 +1732,12 @@ int launch_pcisph_substep(SphCtx *c, cudaStream_t st, SphPcisphStep *io, int64_t
 // message (DX_MISC) and k_iisph_shard_reactions gathers the reactions onto the owned dynamic solids before the advect.
 int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n_grid, int64_t *kernels) {
     const DevParams &P = c->P;
-    const int b128 = blocks_for(n_grid, 128), b256 = blocks_for(n_grid, 256);
-    launch_pair_density(c, st, kernels, /*split_mode=*/0, n_grid);
-    c->list_valid = true;
-    DevParams Pn = P;
-    Pn.sigma = 0.0f;  // IISPH's non-pressure forces are gravity + viscosity: the cohesion term is an exact zero
-    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, c->S);
-    k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 2;
+    solver_densities(c, st, n_grid, kernels);
+    non_pressure_forces(c, st, n_grid, /*cohesion=*/false, kernels);
+    predict_velocity(c, st, n_grid, kernels);
     int rc = shard_dfsph_exchange(c, st, DX_VELD, nullptr, false, kernels);
     if (rc) return rc;
-    k_iisph_predict<<<b128, 128, 0, st>>>(P, c->S);
-    *kernels += 1;
+    iisph_predict(c, st, n_grid, kernels);
     rc = shard_dfsph_exchange(c, st, DX_AUX, nullptr, false, kernels);
     if (rc) return rc;
     DfsphCtrl h{};
@@ -1715,22 +1745,17 @@ int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n
                           kernels);
     if (rc) return rc;
     io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-    if (c->shard == ShardMode::Bodies) {
-        k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, c->S, nullptr);
-        *kernels += 1;
+    const bool bodies = c->shard == ShardMode::Bodies;
+    iisph_pressure_accel(c, st, n_grid, /*reactions=*/!bodies, nullptr, kernels);
+    if (bodies) {
         rc = shard_dfsph_exchange(c, st, DX_MISC, nullptr, false, kernels);
         if (rc) return rc;
         if (P.n_solid > 0) {
             k_iisph_shard_reactions<<<blocks_for((int64_t)P.n_solid * 32, 128), 128, 0, st>>>(P, c->S);
             *kernels += 1;
         }
-    } else {
-        k_iisph_pressure_accel<true><<<b128, 128, 0, st>>>(P, c->S, nullptr);
-        *kernels += 1;
     }
-    k_iisph_advect<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 1;
-    c->built = false; c->list_valid = false;  // positions moved
+    iisph_advect(c, st, n_grid, kernels);
     return SPH_OK;
 }
 
@@ -1744,63 +1769,57 @@ int launch_iisph_substep(SphCtx *c, cudaStream_t st, SphIisphStep *io, int64_t n
 // change: one message carries both, and the scale at the end of the divergence loop needs no message because nothing
 // reads a ghost's factor before the pressure loop's opening exchange.
 int launch_dfsph_substep(SphCtx *c, cudaStream_t st, SphDfsphStep *io, int64_t n_grid, int64_t *kernels) {
-    const DevParams &P = c->P;
-    const int b128 = blocks_for(n_grid, 128), b256 = blocks_for(n_grid, 256);
-    launch_pair_density(c, st, kernels, /*split_mode=*/0, n_grid);
-    c->list_valid = true;
-    k_dfsph_factor<<<b128, 128, 0, st>>>(P, c->S);
-    *kernels += 1;
+    solver_densities(c, st, n_grid, kernels);
+    dfsph_factor(c, st, n_grid, kernels);
     DfsphCtrl h{};
     if (io->enable_divergence_solver) {  // divergence_solve, DFSPH.py:236-276
-        k_dfsph_density_change<0><<<b128, 128, 0, st>>>(P, c->S);
-        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt);
-        *kernels += 2;
+        dfsph_density_change(c, st, n_grid, 0, kernels);
+        dfsph_multiply_factor(c, st, n_grid, io->inv_dt, kernels);
         int rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
         if (rc) return rc;
         rc = dfsph_solve_loop(c, 0, io->max_iterations_v, io->eta_v, 0.0f, io->n_fluid, io->first_batch_v, &h, st, n_grid,
                               kernels);
         if (rc) return rc;
         io->iterations_v = h.iterations; io->avg_err_v = h.last_avg; io->first_batch_v = std::max(1, h.sweeps);
-        k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->dt);
-        *kernels += 1;
+        dfsph_multiply_factor(c, st, n_grid, io->dt, kernels);
     }
-    k_dfsph_non_pressure<<<b128, 128, 0, st>>>(P, c->S);
-    k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 2;
+    non_pressure_forces(c, st, n_grid, /*cohesion=*/true, kernels);
+    predict_velocity(c, st, n_grid, kernels);
     int rc = shard_dfsph_exchange(c, st, DX_VELD, nullptr, false, kernels);
     if (rc) return rc;
     // pressure_solve, DFSPH.py:314-352
-    k_dfsph_density_change<1><<<b128, 128, 0, st>>>(P, c->S);
-    k_dfsph_multiply_factor<<<b256, 256, 0, st>>>(P, c->S, io->inv_dt2);
-    *kernels += 2;
+    dfsph_density_change(c, st, n_grid, 1, kernels);
+    dfsph_multiply_factor(c, st, n_grid, io->inv_dt2, kernels);
     rc = shard_dfsph_exchange(c, st, DX_DFS, nullptr, false, kernels);
     if (rc) return rc;
     rc = dfsph_solve_loop(c, 1, io->max_iterations, io->eta, io->density0, io->n_fluid, io->first_batch, &h, st, n_grid,
                           kernels);
     if (rc) return rc;
     io->iterations = h.iterations; io->avg_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-    k_dfsph_advect<<<b256, 256, 0, st>>>(P, c->S);
-    *kernels += 1;
-    c->built = false; c->list_valid = false;  // positions moved
+    dfsph_advect(c, st, n_grid, kernels);
     return SPH_OK;
 }
 
-// One single-GPU SPHBase.step() (sph_base.py:263-271) of a solver whose substep launches itself (DFSPH, IISPH,
-// PCISPH):
+// The single-GPU step entry points of the solvers whose substep launches itself (DFSPH, IISPH, PCISPH): their mode
+// checks, then nsteps of SPHBase.step() (sph_base.py:263-271):
 //   neighbour build -> moving boundary volumes -> substep() -> solve_rigid_body -> enforce_boundary_3D(fluid)
 template <typename Substep>
-int single_step(SphCtx *ctx, cudaStream_t st, Substep substep) {
-    // ps.initialize_particle_system(), compute_moving_boundary_volume() (sph_base.py:264-265)
-    int rc = launch_neighbor_build(ctx, st, nullptr, &ctx->launches, /*move_acc=*/true);
-    if (rc) return rc;
-    if (ctx->has_dynamic_solids) { rc = launch_boundary_volume(ctx, 1, st, &ctx->launches); if (rc) return rc; }
-    rc = substep();
-    if (rc) return rc;
-    // solve_rigid_body(), enforce_boundary_3D(fluid) (sph_base.py:270-271)
-    if (!ctx->bodies.empty()) { rc = launch_rigid_solve(ctx, st, &ctx->launches); if (rc) return rc; }
-    k_enforce_boundary<<<blocks_for(ctx->P.n, 256), 256, 0, st>>>(ctx->P, ctx->S, /*particle_type=*/1);
-    ctx->launches += 1;
-    CUDA_TRY(ctx, cudaGetLastError());
+int run_single_steps(SphCtx *ctx, cudaStream_t st, int32_t nsteps, const Need &need, bool args_ok, Substep substep) {
+    if (int rc = require(ctx, need, args_ok)) return rc;
+    if (ctx->P.n == 0) return SPH_OK;
+    for (int s = 0; s < nsteps; ++s) {
+        // ps.initialize_particle_system(), compute_moving_boundary_volume() (sph_base.py:264-265)
+        int rc = launch_neighbor_build(ctx, st, nullptr, &ctx->launches, /*move_acc=*/true);
+        if (rc) return rc;
+        if (ctx->has_dynamic_solids) { rc = launch_boundary_volume(ctx, 1, st, &ctx->launches); if (rc) return rc; }
+        rc = substep();
+        if (rc) return rc;
+        // solve_rigid_body(), enforce_boundary_3D(fluid) (sph_base.py:270-271)
+        if (!ctx->bodies.empty()) { rc = launch_rigid_solve(ctx, st, &ctx->launches); if (rc) return rc; }
+        k_enforce_boundary<<<blocks_for(ctx->P.n, 256), 256, 0, st>>>(ctx->P, ctx->S, /*particle_type=*/1);
+        ctx->launches += 1;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
     return SPH_OK;
 }
 
@@ -1843,6 +1862,41 @@ int shard_dfsph_sequence(SphCtx *c, cudaStream_t st, bool wide, int64_t *kernels
 }  // namespace
 extern "C" {
 
+int sph_dfsph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
+    if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph))) return rc;
+    const int64_t n = ctx->P.n;
+    if (n == 0) return SPH_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (op >= DFSPH_COMPUTE_DENSITIES && op <= DFSPH_NON_PRESSURE_FORCES && op != DFSPH_DENSITY_ERROR &&
+        op != DFSPH_MULTIPLY_FACTOR) {
+        if (!ctx->built)
+            return fail(ctx, SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first");
+        if (op != DFSPH_COMPUTE_DENSITIES && !ctx->list_valid)
+            return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run op 0 (compute_densities) first");
+    }
+    int64_t *k = &ctx->launches;
+    switch (op) {
+        case DFSPH_COMPUTE_DENSITIES: solver_densities(ctx, st, n, k); break;
+        case DFSPH_COMPUTE_FACTOR: dfsph_factor(ctx, st, n, k); break;
+        case DFSPH_DENSITY_CHANGE: dfsph_density_change(ctx, st, n, 0, k); break;
+        case DFSPH_DENSITY_ADV: dfsph_density_change(ctx, st, n, 1, k); break;
+        case DFSPH_DENSITY_ERROR:  // the host loop's error read-back; the device loop fuses it into the density change
+            if (!out_dev) return SPH_E_ARG;
+            k_dfsph_density_error<<<blocks_for(n, 256), 256, 0, st>>>(ctx->P, ctx->S, arg, static_cast<double *>(out_dev));
+            *k += 1;
+            break;
+        case DFSPH_MULTIPLY_FACTOR: dfsph_multiply_factor(ctx, st, n, arg, k); break;
+        case DFSPH_DIVERGENCE_ITERATION: dfsph_iteration(ctx, st, n, 0, nullptr, k); break;
+        case DFSPH_PRESSURE_ITERATION: dfsph_iteration(ctx, st, n, 1, nullptr, k); break;
+        case DFSPH_NON_PRESSURE_FORCES: non_pressure_forces(ctx, st, n, /*cohesion=*/true, k); break;
+        case DFSPH_PREDICT_VELOCITY: predict_velocity(ctx, st, n, k); break;
+        case DFSPH_ADVECT: dfsph_advect(ctx, st, n, k); break;
+        default: return fail(ctx, SPH_E_ARG, "unknown DFSPH op");
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    return SPH_OK;
+}
+
 int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double eta, float offset, int64_t n_fluid,
                     int32_t first_batch, int32_t *iterations_out, int32_t *sweeps_out, double *avg_err_out, void *stream) {
     if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph).fresh_lists(), (mode == 0 || mode == 1) && n_fluid >= 1))
@@ -1858,59 +1912,37 @@ int sph_dfsph_solve(SphCtx *ctx, int32_t mode, int32_t max_iterations, double et
 }
 
 int sph_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *stream) {
-    const char *sharded = "this context is sharded: step it with sph_shard_dfsph_step";
-    if (int rc = require(ctx, Need().runs(Solver::DFSPH, kNoDfsph).unsharded(sharded), io && nsteps >= 0 && io->n_fluid >= 1))
-        return rc;
-    if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int s = 0; s < nsteps; ++s) {
-        int rc = single_step(ctx, st, [&] { return launch_dfsph_substep(ctx, st, io, ctx->P.n, &ctx->launches); });
-        if (rc) return rc;
-    }
-    return SPH_OK;
+    const char *sharded = "this context is sharded: step it with sph_shard_dfsph_step";
+    return run_single_steps(ctx, st, nsteps, Need().runs(Solver::DFSPH, kNoDfsph).unsharded(sharded),
+                            io && nsteps >= 0 && io->n_fluid >= 1,
+                            [&] { return launch_dfsph_substep(ctx, st, io, ctx->P.n, &ctx->launches); });
 }
 
 int sph_iisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
     if (int rc = require(ctx, Need().runs(Solver::IISPH, kNoIisph).unsharded(kIisphSharded))) return rc;
-    const DevParams &P = ctx->P;
-    if (P.n == 0) return SPH_OK;
+    const int64_t n = ctx->P.n;
+    if (n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
     if (op < IISPH_COMPUTE_DENSITIES || op > IISPH_ADVECT) return fail(ctx, SPH_E_ARG, "unknown IISPH op");
     if (!ctx->built) return fail(ctx, SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first");
     if (op != IISPH_COMPUTE_DENSITIES && op != IISPH_ADVECT && !ctx->list_valid)
         return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run op 0 (compute_densities) first");
     if (op == IISPH_PRESSURE_SOLVE_ITERATION && !out_dev) return SPH_E_ARG;
-    DevParams Pn = P;
+    int64_t *k = &ctx->launches;
     switch (op) {
-        case IISPH_COMPUTE_DENSITIES:
-            launch_pair_density(ctx, st, &ctx->launches);
-            ctx->list_valid = true;
-            break;
-        case IISPH_NON_PRESSURE_FORCES:
-            Pn.sigma = 0.0f;  // gravity + viscosity only
-            k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, ctx->S);
-            ctx->launches += 1;
-            break;
+        case IISPH_COMPUTE_DENSITIES: solver_densities(ctx, st, n, k); break;
+        case IISPH_NON_PRESSURE_FORCES: non_pressure_forces(ctx, st, n, /*cohesion=*/false, k); break;
         case IISPH_PREDICT_ADVECTION:
-            k_dfsph_predict_velocity<<<b256, 256, 0, st>>>(P, ctx->S);
-            k_iisph_predict<<<b128, 128, 0, st>>>(P, ctx->S);
-            ctx->launches += 2;
+            predict_velocity(ctx, st, n, k);
+            iisph_predict(ctx, st, n, k);
             break;
-        case IISPH_PRESSURE_SOLVE_ITERATION:
-            k_iisph_pressure_accel<false><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
-            k_iisph_pressure_update<<<b128, 128, 0, st>>>(P, ctx->S, arg, static_cast<double *>(out_dev), nullptr);
-            ctx->launches += 2;
+        case IISPH_PRESSURE_SOLVE_ITERATION:  // one sweep of iisph_solve_loop without its check
+            iisph_pressure_accel(ctx, st, n, /*reactions=*/false, nullptr, k);
+            iisph_pressure_update(ctx, st, n, arg, static_cast<double *>(out_dev), nullptr, k);
             break;
-        case IISPH_PRESSURE_FORCES:
-            k_iisph_pressure_accel<true><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
-            ctx->launches += 1;
-            break;
-        case IISPH_ADVECT:
-            k_iisph_advect<<<b256, 256, 0, st>>>(P, ctx->S);
-            ctx->launches += 1;
-            ctx->built = false; ctx->list_valid = false;
-            break;
+        case IISPH_PRESSURE_FORCES: iisph_pressure_accel(ctx, st, n, /*reactions=*/true, nullptr, k); break;
+        case IISPH_ADVECT: iisph_advect(ctx, st, n, k); break;
     }
     CUDA_TRY(ctx, cudaGetLastError());
     return SPH_OK;
@@ -1931,16 +1963,10 @@ int sph_iisph_solve(SphCtx *ctx, int32_t max_iterations, float omega, double eta
 }
 
 int sph_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream) {
-    if (int rc = require(ctx, Need().runs(Solver::IISPH, kNoIisph).unsharded(kIisphSharded),
-                         io && nsteps >= 0 && io->n_fluid >= 1 && io->max_iterations >= 1))
-        return rc;
-    if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int s = 0; s < nsteps; ++s) {
-        int rc = single_step(ctx, st, [&] { return launch_iisph_substep(ctx, st, io, ctx->P.n, &ctx->launches); });
-        if (rc) return rc;
-    }
-    return SPH_OK;
+    return run_single_steps(ctx, st, nsteps, Need().runs(Solver::IISPH, kNoIisph).unsharded(kIisphSharded),
+                            io && nsteps >= 0 && io->n_fluid >= 1 && io->max_iterations >= 1,
+                            [&] { return launch_iisph_substep(ctx, st, io, ctx->P.n, &ctx->launches); });
 }
 
 int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) {
@@ -1954,48 +1980,26 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) 
 
 int sph_pcisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
     if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu))) return rc;
-    const DevParams &P = ctx->P;
-    if (P.n == 0) return SPH_OK;
+    const int64_t n = ctx->P.n;
+    if (n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int b128 = blocks_for(P.n, 128), b256 = blocks_for(P.n, 256);
     if (op < PCISPH_COMPUTE_DENSITIES || op > PCISPH_UPDATE_TIME_STEP) return fail(ctx, SPH_E_ARG, "unknown PCISPH op");
     if (!ctx->built) return fail(ctx, SPH_E_ARG, "neighbour structure is stale: call sph_neighbor_build first");
     if (op != PCISPH_COMPUTE_DENSITIES && op != PCISPH_UPDATE_TIME_STEP && !ctx->list_valid)
         return fail(ctx, SPH_E_ARG, "neighbour lists are stale: run op 0 (compute_densities) first");
     if (op == PCISPH_UPDATE_PRESSURE && !out_dev) return SPH_E_ARG;
-    DevParams Pn = P;
+    int64_t *k = &ctx->launches;
     switch (op) {
-        case PCISPH_COMPUTE_DENSITIES:
-            launch_pair_density(ctx, st, &ctx->launches);
-            ctx->list_valid = true;
-            break;
+        case PCISPH_COMPUTE_DENSITIES: solver_densities(ctx, st, n, k); break;
         case PCISPH_COMPUTE_DELTAS:
-            Pn.sigma = 0.0f;  // gravity + viscosity only
-            k_dfsph_non_pressure<<<b128, 128, 0, st>>>(Pn, ctx->S);
-            k_pcisph_init<<<b256, 256, 0, st>>>(P, ctx->S);
-            ctx->launches += 2;
+            non_pressure_forces(ctx, st, n, /*cohesion=*/false, k);
+            pcisph_init(ctx, st, k);
             break;
-        case PCISPH_POS_VEL_PREDICTION:
-            k_pcisph_predict<<<b256, 256, 0, st>>>(P, ctx->S, nullptr);
-            ctx->launches += 1;
-            break;
-        case PCISPH_UPDATE_PRESSURE:
-            k_pcisph_update_pressure<<<b128, 128, 0, st>>>(P, ctx->S, arg, static_cast<int32_t *>(out_dev), nullptr);
-            ctx->launches += 1;
-            break;
-        case PCISPH_UPDATE_PRESSURE_FORCE:
-            k_pcisph_pressure_force<false><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
-            ctx->launches += 1;
-            break;
-        case PCISPH_COMPUTE_PRESSURE_FORCES:
-            k_pcisph_pressure_force<true><<<b128, 128, 0, st>>>(P, ctx->S, nullptr);
-            ctx->launches += 1;
-            break;
-        case PCISPH_UPDATE_TIME_STEP:
-            k_pcisph_advect<<<b256, 256, 0, st>>>(P, ctx->S);
-            ctx->launches += 1;
-            ctx->built = false; ctx->list_valid = false;
-            break;
+        case PCISPH_POS_VEL_PREDICTION: pcisph_predict(ctx, st, nullptr, k); break;
+        case PCISPH_UPDATE_PRESSURE: pcisph_update_pressure(ctx, st, arg, static_cast<int32_t *>(out_dev), nullptr, k); break;
+        case PCISPH_UPDATE_PRESSURE_FORCE: pcisph_pressure_force(ctx, st, /*reactions=*/false, nullptr, k); break;
+        case PCISPH_COMPUTE_PRESSURE_FORCES: pcisph_pressure_force(ctx, st, /*reactions=*/true, nullptr, k); break;
+        case PCISPH_UPDATE_TIME_STEP: pcisph_advect(ctx, st, k); break;
     }
     CUDA_TRY(ctx, cudaGetLastError());
     return SPH_OK;
@@ -2016,16 +2020,10 @@ int sph_pcisph_solve(SphCtx *ctx, float delta, double eta, int32_t min_iteration
 }
 
 int sph_pcisph_step(SphCtx *ctx, int32_t nsteps, SphPcisphStep *io, void *stream) {
-    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu),
-                         io && nsteps >= 0 && io->max_iterations >= 1))
-        return rc;
-    if (ctx->P.n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    for (int s = 0; s < nsteps; ++s) {
-        int rc = single_step(ctx, st, [&] { return launch_pcisph_substep(ctx, st, io, &ctx->launches); });
-        if (rc) return rc;
-    }
-    return SPH_OK;
+    return run_single_steps(ctx, st, nsteps, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu),
+                            io && nsteps >= 0 && io->max_iterations >= 1,
+                            [&] { return launch_pcisph_substep(ctx, st, io, &ctx->launches); });
 }
 
 int sph_pcisph_read(SphCtx *ctx, float *rho_star, float *p, float *ap, void *stream) {

@@ -76,6 +76,11 @@ class Engine:
             raise RuntimeError(f"{what} failed ({rc}): {self.lib.sph_last_error(self.ctx).decode()}")
         return rc
 
+    def _call(self, symbol, *args):
+        """lib.<symbol>(ctx, *args, stream), checked; a tensor argument passes its device pointer, None a NULL."""
+        args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+        self._check(getattr(self.lib, symbol)(self.ctx, *args, self._stream()), symbol)
+
     def close(self):
         if getattr(self, "ctx", None):
             torch.cuda.synchronize(self.device)
@@ -194,8 +199,7 @@ class Engine:
         self._check(self.lib.sph_set_dfsph(self.ctx, int(bool(enable))), "sph_set_dfsph")
 
     def dfsph_op(self, op, arg=0.0, out=None):
-        self._check(self.lib.sph_dfsph_op(self.ctx, int(op), float(arg), None if out is None else out.data_ptr(),
-                                          self._stream()), "sph_dfsph_op")
+        self._call("sph_dfsph_op", int(op), float(arg), out)
 
     def dfsph_solve(self, mode, max_iterations, eta, offset, n_fluid, first_batch):
         """The Jacobi loop of divergence_solve (mode 0) / pressure_solve (mode 1) with the loop condition on the
@@ -214,8 +218,7 @@ class Engine:
         self._check(self.lib.sph_set_iisph(self.ctx, int(bool(enable))), "sph_set_iisph")
 
     def iisph_op(self, op, arg=0.0, out=None):
-        self._check(self.lib.sph_iisph_op(self.ctx, int(op), float(arg), None if out is None else out.data_ptr(),
-                                          self._stream()), "sph_iisph_op")
+        self._call("sph_iisph_op", int(op), float(arg), out)
 
     def iisph_solve(self, max_iterations, omega, eta, n_fluid, first_batch):
         """pressure_solve's Jacobi loop with the loop condition on the device; returns (iterations, last average
@@ -232,15 +235,13 @@ class Engine:
 
     def iisph_read(self, a_ii=None, s=None, ap=None):
         """a_ii [n], s [n], a^p [n, 3] (float32 tensors on the engine's device, each may be None), sorted order."""
-        ptr = [None if t is None else t.data_ptr() for t in (a_ii, s, ap)]
-        self._check(self.lib.sph_iisph_read(self.ctx, *ptr, self._stream()), "sph_iisph_read")
+        self._call("sph_iisph_read", a_ii, s, ap)
 
     def set_pcisph(self, enable=True):
         self._check(self.lib.sph_set_pcisph(self.ctx, int(bool(enable))), "sph_set_pcisph")
 
     def pcisph_op(self, op, arg=0.0, out=None):
-        self._check(self.lib.sph_pcisph_op(self.ctx, int(op), float(arg), None if out is None else out.data_ptr(),
-                                           self._stream()), "sph_pcisph_op")
+        self._call("sph_pcisph_op", int(op), float(arg), out)
 
     def pcisph_solve(self, delta, eta, min_iterations, max_iterations, first_batch):
         """The prediction-correction loop with its condition on the device; returns (iterations, last max error).
@@ -258,8 +259,7 @@ class Engine:
 
     def pcisph_read(self, rho_star=None, p=None, ap=None):
         """rho* [n], p [n], a^p [n, 3] (float32 tensors on the engine's device, each may be None), sorted order."""
-        ptr = [None if t is None else t.data_ptr() for t in (rho_star, p, ap)]
-        self._check(self.lib.sph_pcisph_read(self.ctx, *ptr, self._stream()), "sph_pcisph_read")
+        self._call("sph_pcisph_read", rho_star, p, ap)
 
     def step(self, nsteps=1):
         self._check(self.lib.sph_step(self.ctx, int(nsteps), self._stream()), "sph_step")

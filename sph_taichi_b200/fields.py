@@ -92,3 +92,25 @@ class ScalarField:
         return np.asarray(self._value)
 
     shape = ()
+
+
+class ScratchField:
+    """Read-only per-particle scratch of a solver's last kernels: argument `which` of the engine method `read`
+    (``iisph_read``: a_ii, s_i, a^p; ``pcisph_read``: rho*, p, a^p), in the public fields' order."""
+
+    def __init__(self, solver, read, which, width):
+        self._solver, self._read, self._which, self._width = solver, read, which, width
+
+    @property
+    def shape(self):
+        return (self._solver.ps.particle_max_num,)
+
+    def to_numpy(self):
+        ps = self._solver.ps
+        ps._push()
+        n = ps.particle_max_num
+        out = torch.zeros((n, 3) if self._width == 3 else (n,), dtype=torch.float32, device=ps.device)
+        args = [None, None, None]
+        args[self._which] = out
+        getattr(ps._engine, self._read)(*args)
+        return out.cpu().numpy()

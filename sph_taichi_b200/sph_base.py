@@ -105,7 +105,35 @@ class SPHBase:
             R, cm = R.cpu().numpy(), self.compute_com_kernel(r_obj_id)
         obj["meshVertices"] = posed_mesh(obj["restPosition"], obj["restCenterOfMass"], R, cm)
 
+    def _update_meshes(self):
+        """The OBJ export's posed meshes after a fused step, which keeps R and the centres of mass on the device."""
+        ps = self.ps
+        if ps.cfg.get_cfg("exportObj"):
+            for oid in ps._body_index:
+                if "restPosition" in ps.object_collection[oid]:
+                    self._update_mesh(oid)
+
     # ---- step (sph_base.py:263-271) ----------------------------------------------------------------
+    # The engine methods of a solver's op-by-op path and of its fused step (DFSPH, IISPH, PCISPH)
+    _ENGINE_OP = _ENGINE_STEP = None
+
+    def _op(self, op, arg=0.0, out=None):
+        self.ps._push()
+        getattr(self.ps._engine, self._ENGINE_OP)(op, arg, out)
+        self.ps._after_engine()
+
+    def _solver_step(self, n, io):
+        """n fused steps of the solver in one library call; io carries the constants in and the counts out, and its
+        sweep counts are the first batches of the next step's loops."""
+        ps = self.ps
+        ps._push()
+        getattr(ps._engine, self._ENGINE_STEP)(n, io)
+        ps._after_engine()
+        self._sweeps_guess = ([int(io.first_batch_v), int(io.first_batch)] if hasattr(io, "first_batch_v")
+                              else int(io.first_batch))
+        self._update_meshes()
+        return io
+
     def _fused_step_ok(self):
         return False
 
@@ -115,10 +143,7 @@ class SPHBase:
             ps._push()
             ps._engine.step(n)
             ps._after_engine()
-            if ps.cfg.get_cfg("exportObj"):
-                for oid in ps._body_index:
-                    if "restPosition" in ps.object_collection[oid]:
-                        self._update_mesh(oid)
+            self._update_meshes()
             return
         for _ in range(n):
             ps.initialize_particle_system()
