@@ -238,10 +238,14 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream);
 /* ---- PCISPH (predictive-corrective incompressible SPH, simulationMethod 1; the legacy engine's pci_* methods) ----
  * These calls implement the 3-D formulation DESIGN.md section 11 states (its deviations from the legacy 2-D code are
  * listed there).  sph_set_pcisph(1) puts a context in PCISPH mode: the density pass has DFSPH semantics (no clamp, no
- * EOS), and the WCSPH, DFSPH and IISPH calls (sph_step, sph_dfsph_*, sph_iisph_*) and every sph_shard_configure* call
- * refuse the context: PCISPH is single-GPU, and sph_set_pcisph(1) is refused on a sharded context.  sph_set_dfsph,
+ * EOS), and the WCSPH, DFSPH and IISPH calls (sph_step, sph_dfsph_*, sph_iisph_*, sph_shard_step,
+ * sph_shard_profile_step, sph_shard_dfsph_step, sph_shard_iisph_step), sph_shard_configure and the body configures
+ * refuse the context.  A PCISPH context may be x-slab sharded (fluid + static solids): sph_set_pcisph(1) BEFORE
+ * sph_shard_configure_pcisph (it is refused on a sharded context), then sph_shard_pcisph_step (below).  sph_set_dfsph,
  * sph_set_iisph(1) or sph_set_pcisph(0) leave the mode (sph_set_pcisph(0) on a context that is not in PCISPH mode
- * changes nothing).  The PCISPH calls refuse a context that is not in PCISPH mode.  One op per method name:
+ * changes nothing).  The PCISPH calls refuse a context that is not in PCISPH mode, and sph_pcisph_op, sph_pcisph_solve
+ * and sph_pcisph_step refuse a sharded one (their grids cover the capacity, ghosts and trash included).  One op per
+ * method name:
  *   0 compute_densities (also builds the neighbour lists)
  *   1 pci_compute_deltas (a^np = gravity + viscosity; p = 0, a^p = 0)
  *   2 pci_pos_vel_prediction (v* = v + dt (a^np + a^p), x* = x + dt v*; solids stay at x^t)
@@ -312,6 +316,11 @@ int sph_pcisph_read(SphCtx *ctx, float *rho_star, float *p, float *ap, void *str
  * every pressure-acceleration pass -- two exchanges per relaxed Jacobi sweep.  With dynamic solids
  * (sph_shard_configure_iisph_bodies) one more word follows the loop: the final pressures (misc.y).
  *
+ * PCISPH contexts (sph_set_pcisph(1), then sph_shard_configure_pcisph; fluid + static solids) step with
+ * sph_shard_pcisph_step: the same step shape, with the outermost owned layer's predicted record {x*, m_V} sent after
+ * every prediction and its pressure (misc.y) after every pressure update -- two exchanges per prediction-correction
+ * sweep, and none outside the loop.
+ *
  * The exchange goes through an SphTransport: NCCL point-to-point (libnccl.so.2 is dlopen'ed; the communicator
  * belongs to this library, created from an id the caller distributes), or caller-supplied functions (the CPU
  * test-suite routes them to torch.distributed / gloo against the host-emulated build); set it before
@@ -364,6 +373,12 @@ int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t 
 int sph_shard_configure_iisph_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers,
                                      int64_t halo_capacity, int32_t rebalance_every, const SphRigidBody *bodies,
                                      int32_t n_bodies);
+/* Opt-in sharding of PCISPH scenes: the arguments, checks and layout of sph_shard_configure, on a context in PCISPH mode
+ * -- sph_set_pcisph(1) must have been called before it; WCSPH, DFSPH and IISPH contexts are refused (they use
+ * sph_shard_configure), and so is a context with dynamic solids (dynamic solids in PCISPH are single-GPU).  The context
+ * then steps with sph_shard_pcisph_step; sph_shard_begin, sph_shard_info and sph_shard_dump work on it as on the others. */
+int sph_shard_configure_pcisph(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                               int32_t rebalance_every);
 /* first sort of the packed particles + the first halo exchange (no physics) */
 int sph_shard_begin(SphCtx *ctx, void *stream);
 /* nsteps sharded SPHBase.step()s (sph_base.py:263-271): asynchronous launches that run ahead of the device (no host
@@ -389,6 +404,18 @@ int sph_shard_dfsph_step(SphCtx *ctx, int32_t nsteps, SphDfsphStep *io, void *st
  * (SPH_SHARD_GRAPH does not apply).  A particle that moves a whole cell layer in x in one step sets
  * SPH_STATUS_SHARD_VELOCITY.  The warm-start pressure travels in the records (misc.y), so migrating particles keep it. */
 int sph_shard_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *stream);
+/* nsteps sharded PCISPH SPHBase.step()s of a context configured by sph_shard_configure_pcisph (fluid + static solids):
+ * the step of sph_pcisph_step with `io` used the same way.  One step:
+ *     plan -> classify + sort -> info -> DX ranges -> ghost alignment -> densities (owned + first ghost layer)
+ *     -> non-pressure forces -> p = 0, a^p = 0, x* = x
+ *     -> loop { prediction -> [dfs = {x*, m_V}] -> predicted density + pressure update (error partial) -> [misc.y = p
+ *               + all-gather of the partials] -> pressure force -> the loop check on the max of the partials }
+ *     -> final pressure force -> advect -> fluid wall clamp -> the record exchange
+ * ([w] as for sph_shard_iisph_step.)  The max of the ranks' partials is exact and independent of order, so every rank
+ * runs the same sweeps and returns the same iterations, first_batch and max_err values (max_err bit-identical).  Eager
+ * launches with one host wait per batch of sweeps (SPH_SHARD_GRAPH does not apply).  A particle that moves a whole
+ * cell layer in x in one step sets SPH_STATUS_SHARD_VELOCITY. */
+int sph_shard_pcisph_step(SphCtx *ctx, int32_t nsteps, SphPcisphStep *io, void *stream);
 /* out2 = {transport groups this context issued from the host, bytes it sent in them}; graph replays of
  * sph_shard_step (SPH_SHARD_GRAPH=1) re-issue the captured groups without counting them */
 int sph_shard_transport_stats(SphCtx *ctx, uint64_t *out2);
@@ -415,7 +442,7 @@ int sph_shard_info(SphCtx *ctx, int32_t *out16, uint64_t *out_sent, void *stream
  * rank's status word (sph_shard_info's), the same on every rank, also when SPH_E_CAPACITY is returned.
  * sph_shard_transport_stats counts the bytes like any other group: this rank sends (world - 1) * 16 bytes of headers,
  * plus, on ranks other than rank 0, 24 bytes (x and v, 3 float32 each) per row it holds.  Launches nothing into
- * sph_shard_step's graphs; works on WCSPH, DFSPH, IISPH and sph_shard_configure_bodies contexts.  Single-GPU contexts are
+ * sph_shard_step's graphs; works on WCSPH, DFSPH, IISPH, PCISPH and sph_shard_configure_bodies contexts.  Single-GPU contexts are
  * refused (they have sph_unpack_xv); capacity < 0 or a null pointer returns SPH_E_ARG. */
 int sph_shard_dump(SphCtx *ctx, int32_t object_id, float *x, float *v, int64_t capacity, int64_t *rows_out,
                    uint32_t *status_out, void *stream);

@@ -14,7 +14,8 @@ The loop and the output files are those of the single-GPU run; rank 0 writes the
 gathers object 0 over the engine's own transport; the torch process group, gloo, only carries the NCCL id).
 `--gpus 1` runs the sharded engine on one GPU without torch.distributed.run.  IISPH scenes (simulationMethod 3) shard
 only on request, `--gpus N --shard-iisph`; without the flag they are refused.  IISPH scenes with dynamic solids need
-`--gpus N --shard-iisph-bodies` (which implies `--shard-iisph`).
+`--gpus N --shard-iisph-bodies` (which implies `--shard-iisph`).  PCISPH scenes (simulationMethod 1, fluid and static
+solids) shard only on request too, `--gpus N --shard-pcisph`.
 """
 import argparse
 import copy
@@ -99,13 +100,14 @@ def _resolved_scene(config):
     return sc
 
 
-def run_sharded(config, scene_name, frames, device, transport=None, quiet=False, iisph=False, iisph_bodies=False):
+def run_sharded(config, scene_name, frames, device, transport=None, quiet=False, iisph=False, iisph_bodies=False,
+                pcisph=False):
     """The same loop and output files as `run_single`, on the x-slab sharded engine: this process is rank RANK of
     WORLD_SIZE (environment, default 0 of 1) on `device`.  Every rank steps and joins each `dump`; rank 0 writes the
     files and prints the summary.  `transport`: an SphTransport object in place of the library's NCCL communicator
     (slab.GlooTransport); with world > 1 and no transport the torch process group must be initialised.  `iisph`:
     shard an IISPH scene (`slab.build_sharded(..., iisph=True)`); `iisph_bodies`: one with dynamic solids
-    (`iisph_bodies=True`)."""
+    (`iisph_bodies=True`); `pcisph`: shard a PCISPH scene (`pcisph=True`)."""
     from sph_taichi_b200 import slab
     from sph_taichi_b200.sph_base import posed_mesh
 
@@ -114,7 +116,7 @@ def run_sharded(config, scene_name, frames, device, transport=None, quiet=False,
     try:
         sim, n_total = slab.build_sharded(_resolved_scene(config), rank, world, device, transport=transport,
                                           dynamic_solids=slab.scene_has_dynamic_solids(config), iisph=iisph,
-                                          iisph_bodies=iisph_bodies)
+                                          iisph_bodies=iisph_bodies, pcisph=pcisph)
     except NotImplementedError as exc:
         raise SystemExit(f"{scene_name}: {exc}") from exc
     substeps = config.get_cfg("numberOfStepsPerRenderUpdate")
@@ -174,7 +176,7 @@ def main_sharded(args, config, scene_name):
         dist.init_process_group("gloo", rank=rank, world_size=world)  # carries the NCCL id only
     try:
         return run_sharded(config, scene_name, args.frames, dev, quiet=args.quiet, iisph=args.shard_iisph,
-                           iisph_bodies=args.shard_iisph_bodies)
+                           iisph_bodies=args.shard_iisph_bodies, pcisph=args.shard_pcisph)
     finally:
         if world > 1:
             dist.destroy_process_group()
@@ -193,11 +195,15 @@ if __name__ == "__main__":
                         help="with --gpus: shard an IISPH scene (simulationMethod 3; fluid and static solids)")
     parser.add_argument("--shard-iisph-bodies", action="store_true",
                         help="with --gpus: shard an IISPH scene with dynamic solids (implies --shard-iisph)")
+    parser.add_argument("--shard-pcisph", action="store_true",
+                        help="with --gpus: shard a PCISPH scene (simulationMethod 1; fluid and static solids)")
     args = parser.parse_args()
     if args.shard_iisph_bodies and args.gpus is None:
         parser.error("--shard-iisph-bodies needs --gpus N")
     if args.shard_iisph and args.gpus is None:
         parser.error("--shard-iisph needs --gpus N")
+    if args.shard_pcisph and args.gpus is None:
+        parser.error("--shard-pcisph needs --gpus N")
     if args.scene:
         from sph_taichi_b200 import scene as _scene
         scene_path = args.scene + ".json"

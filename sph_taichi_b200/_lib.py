@@ -30,6 +30,7 @@ ABI_SYMBOLS = [
     "sph_shard_transport_stats", "sph_shard_configure_bodies", "sph_shard_dump", "sph_set_iisph", "sph_iisph_op",
     "sph_iisph_solve", "sph_iisph_step", "sph_iisph_read", "sph_shard_iisph_step", "sph_shard_configure_iisph_bodies",
     "sph_set_pcisph", "sph_pcisph_op", "sph_pcisph_solve", "sph_pcisph_step", "sph_pcisph_read",
+    "sph_shard_configure_pcisph", "sph_shard_pcisph_step",
 ]
 
 
@@ -188,6 +189,8 @@ def load():
                                        vp]),
         "sph_pcisph_step": (C.c_int, [vp, i32, C.POINTER(SphPcisphStep), vp]),
         "sph_pcisph_read": (C.c_int, [vp, vp, vp, vp, vp]),
+        "sph_shard_configure_pcisph": (C.c_int, [vp, i32, i32, i32, i64, i32]),
+        "sph_shard_pcisph_step": (C.c_int, [vp, i32, C.POINTER(SphPcisphStep), vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

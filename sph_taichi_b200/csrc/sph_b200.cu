@@ -51,10 +51,21 @@ const char *const kNoDfsph = "sph_set_dfsph(1) was not called";
 const char *const kNoIisph = "sph_set_iisph(1) was not called";
 const char *const kPcisphContext =
     "this context is in PCISPH mode (sph_set_pcisph): it steps with sph_pcisph_op / sph_pcisph_solve / sph_pcisph_step";
-// the PCISPH calls launch over all records and exchange nothing: PCISPH is single-GPU
+// sph_shard_configure and the body configures refuse a PCISPH context, and sph_set_pcisph(1) a sharded one: a PCISPH
+// context shards through sph_shard_configure_pcisph only, in PCISPH mode from the start
 const char *const kPcisphSingleGpu =
     "PCISPH (sph_set_pcisph) is single-GPU: x-slab sharding runs WCSPH, DFSPH and IISPH contexts";
 const char *const kNoPcisph = "sph_set_pcisph(1) was not called";
+// sharded PCISPH (sph_shard_pcisph_step) runs fluid and static solids; the single-GPU PCISPH calls launch over the
+// capacity of a sharded context and would step its ghost and trash records too
+const char *const kPcisphSharded = "this PCISPH context is sharded: step it with sph_shard_pcisph_step";
+const char *const kPcisphShardStep =
+    "this context is in PCISPH mode (sph_set_pcisph): a sharded PCISPH context steps with sph_shard_pcisph_step";
+const char *const kShardPcisphContext =
+    "sph_shard_configure_pcisph shards a PCISPH context: call sph_set_pcisph(1) before it (WCSPH, DFSPH and IISPH "
+    "contexts use sph_shard_configure)";
+const char *const kShardBodiesPcisph =
+    "x-slab sharding of a PCISPH context runs fluid and static solids: dynamic solids in PCISPH are single-GPU";
 const char *const kWorldChanged = "the transport's world size changed after sph_shard_configure: configure again";
 // device copy P.dfsph, set for IISPH and PCISPH too: the three list-based solvers share the density pass (no clamp,
 // no EOS)
@@ -261,15 +272,15 @@ struct Need {
 
 // The mode checks of every entry point, in this order: configured, the entry point's bare argument checks (args_ok),
 // solver, not sharded, not a body context, begun, world size unchanged, then the neighbour structure; returns the first
-// refusal or SPH_OK.  Other solvers' entry points refuse an IISPH context with one message per kind (sharded or not),
-// and a PCISPH context (never sharded) with one message.
+// refusal or SPH_OK.  Other solvers' entry points refuse an IISPH or a PCISPH context with one message per kind (sharded
+// or not).
 int require(SphCtx *c, const Need &n, bool args_ok = true) {
     if (!c) return SPH_E_ARG;
     if (n.configured && c->shard == ShardMode::Off) return fail(c, SPH_E_ARG, "sph_shard_configure was not called");
     if (!args_ok) return SPH_E_ARG;
     if (n.other_solver && c->solver != n.solver)
         return fail(c, SPH_E_ARG, c->solver == Solver::IISPH    ? (n.configured ? kIisphShardStep : kIisphContext)
-                                  : c->solver == Solver::PCISPH ? kPcisphContext
+                                  : c->solver == Solver::PCISPH ? (n.configured ? kPcisphShardStep : kPcisphContext)
                                                                 : n.other_solver);
     if (n.if_sharded && c->shard != ShardMode::Off) return fail(c, SPH_E_ARG, n.if_sharded);
     if (n.if_bodies && c->shard == ShardMode::Bodies) return fail(c, SPH_E_ARG, n.if_bodies);
@@ -1252,6 +1263,19 @@ int sph_shard_configure(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_l
     return shard_setup(ctx, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, 0);
 }
 
+int sph_shard_configure_pcisph(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
+                               int32_t rebalance_every) {
+    if (!ctx) return SPH_E_ARG;
+    if (ctx->solver != Solver::PCISPH) return fail(ctx, SPH_E_ARG, kShardPcisphContext);
+    // PCISPH scatters the reactions onto dynamic solids once per step, after its loop: a reaction gather like IISPH's
+    // would carry over, but it is not written
+    const bool dynamic = !ctx->bodies.empty() || (ctx->P.n_solid > 0 && ctx->has_dynamic_solids);
+    if (int rc = check_slab_args(ctx, false, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every,
+                                 dynamic ? kShardBodiesPcisph : nullptr))
+        return rc;
+    return shard_setup(ctx, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, 0);
+}
+
 int sph_shard_configure_bodies(SphCtx *ctx, int32_t x_lo, int32_t x_hi, int32_t ghost_layers, int64_t halo_capacity,
                                int32_t rebalance_every, const SphRigidBody *bodies, int32_t n_bodies) {
     return shard_configure_bodies(ctx, false, x_lo, x_hi, ghost_layers, halo_capacity, rebalance_every, bodies, n_bodies);
@@ -1528,7 +1552,7 @@ int shard_dfsph_exchange(SphCtx *c, cudaStream_t st, int what, DfsphCtrl *ctrl, 
 
 // ---- solver stages ------------------------------------------------------------------------
 // One launcher per stage of DFSPH, IISPH and PCISPH, shared by their ops, substeps and device-loop sweeps: it launches
-// the stage over the sorted records [0, n_grid) (PCISPH: all P.n), counts its kernels into *kernels and applies the
+// the stage over the sorted records [0, n_grid), counts its kernels into *kernels and applies the
 // stage's change to the neighbour state.  Launchers never exchange: on a sharded context the substeps and sweeps issue
 // the halo messages between them.  ctrl (may be NULL): a device loop's control block.  reactions: the pressure forces
 // of compute_pressure_forces, which also scatter the reactions onto dynamic solids.
@@ -1591,26 +1615,28 @@ void iisph_advect(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) 
     *kernels += 1;
     c->built = false; c->list_valid = false;  // positions moved
 }
-void pcisph_init(SphCtx *c, cudaStream_t st, int64_t *kernels) {
-    k_pcisph_init<<<blocks_for(c->P.n, 256), 256, 0, st>>>(c->P, c->S);
+void pcisph_init(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    k_pcisph_init<<<blocks_for(n_grid, 256), 256, 0, st>>>(c->P, c->S);
     *kernels += 1;
 }
-void pcisph_predict(SphCtx *c, cudaStream_t st, DfsphCtrl *ctrl, int64_t *kernels) {
-    k_pcisph_predict<<<blocks_for(c->P.n, 256), 256, 0, st>>>(c->P, c->S, ctrl);
+void pcisph_predict(SphCtx *c, cudaStream_t st, int64_t n_grid, DfsphCtrl *ctrl, int64_t *kernels) {
+    k_pcisph_predict<<<blocks_for(n_grid, 256), 256, 0, st>>>(c->P, c->S, ctrl);
     *kernels += 1;
 }
-void pcisph_update_pressure(SphCtx *c, cudaStream_t st, float delta, int32_t *err_max, DfsphCtrl *ctrl,
-                            int64_t *kernels) {
-    k_pcisph_update_pressure<<<blocks_for(c->P.n, 128), 128, 0, st>>>(c->P, c->S, delta, err_max, ctrl);
+// err_part: a sharded loop's fp64 partial of the error max (NULL otherwise)
+void pcisph_update_pressure(SphCtx *c, cudaStream_t st, int64_t n_grid, float delta, int32_t *err_max, double *err_part,
+                            DfsphCtrl *ctrl, int64_t *kernels) {
+    k_pcisph_update_pressure<<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, delta, err_max, err_part, ctrl);
     *kernels += 1;
 }
-void pcisph_pressure_force(SphCtx *c, cudaStream_t st, bool reactions, DfsphCtrl *ctrl, int64_t *kernels) {
-    if (reactions) k_pcisph_pressure_force<true><<<blocks_for(c->P.n, 128), 128, 0, st>>>(c->P, c->S, ctrl);
-    else k_pcisph_pressure_force<false><<<blocks_for(c->P.n, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+void pcisph_pressure_force(SphCtx *c, cudaStream_t st, int64_t n_grid, bool reactions, DfsphCtrl *ctrl,
+                           int64_t *kernels) {
+    if (reactions) k_pcisph_pressure_force<true><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, ctrl);
+    else k_pcisph_pressure_force<false><<<blocks_for(n_grid, 128), 128, 0, st>>>(c->P, c->S, ctrl);
     *kernels += 1;
 }
-void pcisph_advect(SphCtx *c, cudaStream_t st, int64_t *kernels) {
-    k_pcisph_advect<<<blocks_for(c->P.n, 256), 256, 0, st>>>(c->P, c->S);
+void pcisph_advect(SphCtx *c, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
+    k_pcisph_advect<<<blocks_for(n_grid, 256), 256, 0, st>>>(c->P, c->S);
     *kernels += 1;
     c->built = false; c->list_valid = false;  // positions moved
 }
@@ -1689,36 +1715,50 @@ int iisph_solve_loop(SphCtx *ctx, int32_t max_iterations, float omega, double et
     });
 }
 
-// The prediction-correction loop of PCISPH as a device_loop: per sweep k_pcisph_predict, k_pcisph_update_pressure (error
-// max fused), k_pcisph_pressure_force<false> and k_pcisph_check.  Single-GPU: over all n records.
+// The prediction-correction loop of PCISPH over the sorted records [0, n_grid) as a device_loop: per sweep
+// k_pcisph_predict, k_pcisph_update_pressure (error max fused), k_pcisph_pressure_force<false> and k_pcisph_check.
+// Sharded (P.slab_on): every sweep also sends the outermost owned layer's dfs = {x*, m_V} after the prediction and its
+// misc.y = p after the pressure update to the neighbours' first ghost layer -- the two words of a neighbour the
+// pressure force reads -- and all-gathers the fp64 error partials (ctrl->err) for k_pcisph_check_ranked.
 int pcisph_solve_loop(SphCtx *ctx, float delta, double eta, int32_t min_iterations, int32_t max_iterations,
-                      int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t *kernels) {
+                      int32_t first_batch, DfsphCtrl *h, cudaStream_t st, int64_t n_grid, int64_t *kernels) {
     const double threshold = eta * (double)ctx->P.rho0;
+    const bool ranked = ctx->P.slab_on != 0;
     return device_loop(ctx, first_batch, h, st, [&](DfsphCtrl *ctrl) {
-        pcisph_predict(ctx, st, ctrl, kernels);
-        pcisph_update_pressure(ctx, st, delta, &ctrl->err_max, ctrl, kernels);
-        pcisph_pressure_force(ctx, st, /*reactions=*/false, ctrl, kernels);
-        k_pcisph_check<<<1, 1, 0, st>>>(ctrl, threshold, min_iterations, max_iterations);
+        pcisph_predict(ctx, st, n_grid, ctrl, kernels);
+        int rc = shard_dfsph_exchange(ctx, st, DX_DFS, ctrl, false, kernels);
+        if (rc) return rc;
+        pcisph_update_pressure(ctx, st, n_grid, delta, &ctrl->err_max, ranked ? &ctrl->err : nullptr, ctrl, kernels);
+        rc = shard_dfsph_exchange(ctx, st, DX_MISC, ctrl, true, kernels);
+        if (rc) return rc;
+        pcisph_pressure_force(ctx, st, n_grid, /*reactions=*/false, ctrl, kernels);
+        if (ranked)
+            k_pcisph_check_ranked<<<1, 1, 0, st>>>(ctrl, shard_err_parts(ctx), ctx->rank, ctx->world, threshold,
+                                                   min_iterations, max_iterations);
+        else
+            k_pcisph_check<<<1, 1, 0, st>>>(ctrl, threshold, min_iterations, max_iterations);
         *kernels += 1;
         return SPH_OK;
     });
 }
 
-// The PCISPH substep (DESIGN section 11): densities (+ lists) -> pci_compute_deltas (non-pressure forces without
-// cohesion, then p = 0, a^p = 0) -> the prediction-correction loop -> compute_pressure_forces (the last sweep's a^p
-// again, now with the reactions on dynamic solids: once per step, after the loop) -> pci_update_time_step.  io:
-// constants in, counts out.
-int launch_pcisph_substep(SphCtx *c, cudaStream_t st, SphPcisphStep *io, int64_t *kernels) {
-    solver_densities(c, st, c->P.n, kernels);
-    non_pressure_forces(c, st, c->P.n, /*cohesion=*/false, kernels);
-    pcisph_init(c, st, kernels);
+// The PCISPH substep (DESIGN section 11) over the sorted records [0, n_grid): densities (+ lists) -> pci_compute_deltas
+// (non-pressure forces without cohesion, then p = 0, a^p = 0) -> the prediction-correction loop ->
+// compute_pressure_forces (the last sweep's a^p again, now with the reactions on dynamic solids: once per step, after
+// the loop) -> pci_update_time_step.  io: constants in, counts out.  Sharded (fluid and static solids), the loop's two
+// exchanges per sweep are the only messages: compute_pressure_forces reads the words the last executed sweep sent, and
+// there are no reactions.
+int launch_pcisph_substep(SphCtx *c, cudaStream_t st, SphPcisphStep *io, int64_t n_grid, int64_t *kernels) {
+    solver_densities(c, st, n_grid, kernels);
+    non_pressure_forces(c, st, n_grid, /*cohesion=*/false, kernels);
+    pcisph_init(c, st, n_grid, kernels);
     DfsphCtrl h{};
     int rc = pcisph_solve_loop(c, io->delta, io->eta, io->min_iterations, io->max_iterations, io->first_batch, &h, st,
-                               kernels);
+                               n_grid, kernels);
     if (rc) return rc;
     io->iterations = h.iterations; io->max_err = h.last_avg; io->first_batch = std::max(1, h.sweeps);
-    pcisph_pressure_force(c, st, /*reactions=*/true, nullptr, kernels);
-    pcisph_advect(c, st, kernels);
+    pcisph_pressure_force(c, st, n_grid, /*reactions=*/true, nullptr, kernels);
+    pcisph_advect(c, st, n_grid, kernels);
     return SPH_OK;
 }
 
@@ -1823,7 +1863,7 @@ int run_single_steps(SphCtx *ctx, cudaStream_t st, int32_t nsteps, const Need &n
     return SPH_OK;
 }
 
-// One sharded SPHBase.step() of a solver whose substep launches itself (DFSPH, IISPH; no overlap of the exchanges with
+// One sharded SPHBase.step() of a solver whose substep launches itself (DFSPH, IISPH, PCISPH; no overlap of the exchanges with
 // computation):
 //   shard_sort -> DX ranges -> ghost alignment [-> solid-id slot map -> moving boundary volumes]
 //   -> substep(n_grid) on owned records + ghosts [-> body all-gather + solve -> clamps of the other dynamic solids]
@@ -1979,7 +2019,7 @@ int sph_iisph_read(SphCtx *ctx, float *a_ii, float *s, float *ap, void *stream) 
 }
 
 int sph_pcisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *stream) {
-    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu))) return rc;
+    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSharded))) return rc;
     const int64_t n = ctx->P.n;
     if (n == 0) return SPH_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1993,13 +2033,15 @@ int sph_pcisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *strea
         case PCISPH_COMPUTE_DENSITIES: solver_densities(ctx, st, n, k); break;
         case PCISPH_COMPUTE_DELTAS:
             non_pressure_forces(ctx, st, n, /*cohesion=*/false, k);
-            pcisph_init(ctx, st, k);
+            pcisph_init(ctx, st, n, k);
             break;
-        case PCISPH_POS_VEL_PREDICTION: pcisph_predict(ctx, st, nullptr, k); break;
-        case PCISPH_UPDATE_PRESSURE: pcisph_update_pressure(ctx, st, arg, static_cast<int32_t *>(out_dev), nullptr, k); break;
-        case PCISPH_UPDATE_PRESSURE_FORCE: pcisph_pressure_force(ctx, st, /*reactions=*/false, nullptr, k); break;
-        case PCISPH_COMPUTE_PRESSURE_FORCES: pcisph_pressure_force(ctx, st, /*reactions=*/true, nullptr, k); break;
-        case PCISPH_UPDATE_TIME_STEP: pcisph_advect(ctx, st, k); break;
+        case PCISPH_POS_VEL_PREDICTION: pcisph_predict(ctx, st, n, nullptr, k); break;
+        case PCISPH_UPDATE_PRESSURE:
+            pcisph_update_pressure(ctx, st, n, arg, static_cast<int32_t *>(out_dev), nullptr, nullptr, k);
+            break;
+        case PCISPH_UPDATE_PRESSURE_FORCE: pcisph_pressure_force(ctx, st, n, /*reactions=*/false, nullptr, k); break;
+        case PCISPH_COMPUTE_PRESSURE_FORCES: pcisph_pressure_force(ctx, st, n, /*reactions=*/true, nullptr, k); break;
+        case PCISPH_UPDATE_TIME_STEP: pcisph_advect(ctx, st, n, k); break;
     }
     CUDA_TRY(ctx, cudaGetLastError());
     return SPH_OK;
@@ -2007,12 +2049,12 @@ int sph_pcisph_op(SphCtx *ctx, int32_t op, float arg, void *out_dev, void *strea
 
 int sph_pcisph_solve(SphCtx *ctx, float delta, double eta, int32_t min_iterations, int32_t max_iterations,
                      int32_t first_batch, int32_t *iterations_out, double *max_err_out, void *stream) {
-    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu).fresh_lists(),
+    if (int rc = require(ctx, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSharded).fresh_lists(),
                          max_iterations >= 1))
         return rc;
     DfsphCtrl h{};
     int rc = pcisph_solve_loop(ctx, delta, eta, min_iterations, max_iterations, first_batch, &h,
-                               static_cast<cudaStream_t>(stream), &ctx->launches);
+                               static_cast<cudaStream_t>(stream), ctx->P.n, &ctx->launches);
     if (rc) return rc;
     if (iterations_out) *iterations_out = h.iterations;
     if (max_err_out) *max_err_out = h.last_avg;
@@ -2021,9 +2063,9 @@ int sph_pcisph_solve(SphCtx *ctx, float delta, double eta, int32_t min_iteration
 
 int sph_pcisph_step(SphCtx *ctx, int32_t nsteps, SphPcisphStep *io, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return run_single_steps(ctx, st, nsteps, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSingleGpu),
+    return run_single_steps(ctx, st, nsteps, Need().runs(Solver::PCISPH, kNoPcisph).unsharded(kPcisphSharded),
                             io && nsteps >= 0 && io->max_iterations >= 1,
-                            [&] { return launch_pcisph_substep(ctx, st, io, &ctx->launches); });
+                            [&] { return launch_pcisph_substep(ctx, st, io, ctx->P.n, &ctx->launches); });
 }
 
 int sph_pcisph_read(SphCtx *ctx, float *rho_star, float *p, float *ap, void *stream) {
@@ -2053,6 +2095,16 @@ int sph_shard_iisph_step(SphCtx *ctx, int32_t nsteps, SphIisphStep *io, void *st
                            io && nsteps >= 0 && io->n_fluid >= 1 && io->max_iterations >= 1, [&](bool wide) {
         return shard_dfsph_sequence(ctx, st, wide, &ctx->launches,
                                     [&](int64_t n_grid) { return launch_iisph_substep(ctx, st, io, n_grid, &ctx->launches); });
+    });
+}
+
+int sph_shard_pcisph_step(SphCtx *ctx, int32_t nsteps, SphPcisphStep *io, void *stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    Need need = Need().shard_step(Solver::PCISPH, "sph_set_pcisph(1) was not called before sph_shard_configure_pcisph");
+    return run_shard_steps(ctx, nsteps, need.same_world(kWorldChanged), io && nsteps >= 0 && io->max_iterations >= 1,
+                           [&](bool wide) {
+        return shard_dfsph_sequence(ctx, st, wide, &ctx->launches,
+                                    [&](int64_t n_grid) { return launch_pcisph_substep(ctx, st, io, n_grid, &ctx->launches); });
     });
 }
 

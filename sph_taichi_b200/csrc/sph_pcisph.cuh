@@ -1,6 +1,6 @@
 // sph_pcisph.cuh -- predictive-corrective incompressible SPH (simulationMethod 1; Solenthaler & Pajarola 2009, the
 // reference's legacy engine/sph_solver.py pci_* methods) on top of the same sorted SoA state and per-step neighbour
-// lists as the DFSPH path.  Single-GPU.
+// lists as the DFSPH path.
 //
 // The legacy PCISPH is 2-D code with a racy error estimate, so these kernels implement the 3-D formulation of DESIGN
 // section 11 with its constants.  Per step: the DFSPH density pass (no clamp, no EOS; builds the lists at x^t),
@@ -8,6 +8,13 @@
 // prediction-correction loop (k_pcisph_predict + k_pcisph_update_pressure + k_pcisph_pressure_force<false> +
 // k_pcisph_check per sweep), k_pcisph_pressure_force<true> (the final a^p + reactions on dynamic solids),
 // k_pcisph_advect (pci_update_time_step).
+// x-slab sharded (P.slab_on, sph_shard_pcisph_step; fluid and static solids): every kernel but the density pass works on
+// the owned records.  What a sweep reads of the first ghost layer arrives with the exchanges of the outermost owned
+// layer that the host issues after the kernel that changes it: dfs = {x*, m_V} after k_pcisph_predict (DX_DFS; a
+// solid's word is the x^t k_pcisph_init set) and misc.y = p after k_pcisph_update_pressure (DX_MISC).  Nothing else of
+// a ghost is read after the alignment -- the first sweep's pressure update reads no neighbour p, and the final pressure
+// force reads the last sweep's words -- so no once-per-step message precedes the loop.  The sweep's error is the max
+// over the ranks' fp64 partials (k_pcisph_check_ranked).
 //
 // Per-step scratch, all in existing per-step workspace (no new sorted payload):
 //   acc[i]    = {a^np_i, 0}: gravity + viscosity (fluid); g or 0 (+ reactions) for a solid
@@ -105,11 +112,27 @@ __global__ void k_pcisph_predict(DevParams P, DevArrays S, const DfsphCtrl *ctrl
     S.dfs[i] = make_float4(fmaf(P.dt, v.x, x.x), fmaf(P.dt, v.y, x.y), fmaf(P.dt, v.z, x.z), x.w);
 }
 
+// This rank's error max as an fp64 partial: the bits of the exactly converted double, maxed as an unsigned integer
+// (non-negative doubles order as their bits, a NaN's above every number), so the partial is exact and independent of
+// order.  m = a warp's max of the float bits.
+__device__ __forceinline__ void pcisph_max_partial(double *part, int32_t m) {
+    const double e = (double)__int_as_float(m);
+#ifdef SPH_EMU  // the host emulation has no 64-bit atomicMax
+    uint64_t b, *u = reinterpret_cast<uint64_t *>(part);
+    std::memcpy(&b, &e, 8);
+    uint64_t old = __atomic_load_n(u, __ATOMIC_SEQ_CST);
+    while (old < b && !__atomic_compare_exchange_n(u, &old, b, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {}
+#else
+    atomicMax(reinterpret_cast<unsigned long long *>(part), (unsigned long long)__double_as_longlong(e));
+#endif
+}
+
 // b. pci_update_pressure, with the sweep's error max fused in:
 //   rho*_i = rho0 (m_V_i W(0) + sum_{F+B} m_V_j W(x*_i - x*_j)),  e_i = max(rho*_i - rho0, 0),  p_i <- p_i + delta e_i
 //   err_max = max_i e_i as the int bits of the non-negative float (exact, independent of order)
+// err_part (sharded loops; NULL otherwise): the same max as this rank's fp64 partial (pcisph_max_partial)
 __global__ void __launch_bounds__(128) k_pcisph_update_pressure(DevParams P, DevArrays S, float delta, int32_t *err_max,
-                                                                const DfsphCtrl *ctrl) {
+                                                                double *err_part, const DfsphCtrl *ctrl) {
     if (ctrl && ctrl->done) return;  // written only by k_pcisph_check, between kernels: uniform over the grid
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t fl;
@@ -128,7 +151,10 @@ __global__ void __launch_bounds__(128) k_pcisph_update_pressure(DevParams P, Dev
         S.aux[i].w = rho;
     }
     const int m = __reduce_max_sync(0xffffffffu, __float_as_int(e));
-    if ((threadIdx.x & 31) == 0 && m > 0) atomicMax(err_max, m);
+    if ((threadIdx.x & 31) == 0 && m > 0) {
+        atomicMax(err_max, m);
+        if (err_part) pcisph_max_partial(err_part, m);
+    }
 }
 
 // c. pci_update_pressure_force (REACT = false) and compute_pressure_forces (REACT = true):
@@ -170,18 +196,34 @@ __global__ void __launch_bounds__(128) k_pcisph_pressure_force(DevParams P, DevA
 // The loop of the prediction-correction step, evaluated on the device after every sweep:
 //   it = 0;  do { sweep();  it += 1 } while (!((err < eta rho0 and it >= min_iterations) or it >= max_iterations))
 // threshold = eta rho0 in fp64; err = the sweep's max error, last_avg keeps it.
-__global__ void k_pcisph_check(DfsphCtrl *ctrl, double threshold, int32_t min_iterations, int32_t max_iterations) {
-    if (ctrl->done) return;
-    const float err = __int_as_float(ctrl->err_max);
-    ctrl->last_avg = (double)err;
+__device__ __forceinline__ void pcisph_check_max(DfsphCtrl *ctrl, double err, double threshold, int32_t min_iterations,
+                                                 int32_t max_iterations) {
+    ctrl->last_avg = err;
     ctrl->err_max = 0;
     ctrl->sweeps += 1;
     ctrl->iterations = ctrl->sweeps;
-    if (((double)err < threshold && ctrl->sweeps >= min_iterations) || ctrl->sweeps >= max_iterations) ctrl->done = 1;
+    if ((err < threshold && ctrl->sweeps >= min_iterations) || ctrl->sweeps >= max_iterations) ctrl->done = 1;
+}
+__global__ void k_pcisph_check(DfsphCtrl *ctrl, double threshold, int32_t min_iterations, int32_t max_iterations) {
+    if (ctrl->done) return;
+    pcisph_check_max(ctrl, (double)__int_as_float(ctrl->err_max), threshold, min_iterations, max_iterations);
+}
+// Sharded: parts = the all-gathered fp64 partials of the other ranks, this rank's own still in ctrl->err.  Their max
+// (a NaN in any of them wins, as in the integer max of one rank) is exact and does not depend on the order, so every
+// rank takes the same decision after the same sweep and keeps the same last_avg bits.
+__global__ void k_pcisph_check_ranked(DfsphCtrl *ctrl, const double *parts, int32_t rank, int32_t world,
+                                      double threshold, int32_t min_iterations, int32_t max_iterations) {
+    if (ctrl->done) return;
+    double err = ctrl->err;
+    for (int r = 0; r < world; ++r)
+        if (r != rank && !(err != err || parts[r] <= err)) err = parts[r];
+    ctrl->err = 0.0;
+    pcisph_check_max(ctrl, err, threshold, min_iterations, max_iterations);
 }
 
 // pci_update_time_step: fluid v = v + dt (a^np + a^p), x = x + dt v with the final a^p; a dynamic solid integrates
-// g + reactions as k_dfsph_advect does
+// g + reactions as k_dfsph_advect does.  Sharded: a particle that moves a whole cell layer in x in one step is flagged
+// (SPH_STATUS_SHARD_VELOCITY), as in k_dfsph_advect.
 __global__ void k_pcisph_advect(DevParams P, DevArrays S) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (!dfsph_in_range(P, S, i)) return;
@@ -195,6 +237,7 @@ __global__ void k_pcisph_advect(DevParams P, DevArrays S) {
         v.x += P.dt * a.x; v.y += P.dt * a.y; v.z += P.dt * a.z;
     }
     S.veld[i] = v;
+    if (P.slab_on && !(fabsf(v.x) * P.dt < P.h)) atomicOr(S.status, SPH_STATUS_SHARD_VELOCITY);
     p.x += P.dt * v.x; p.y += P.dt * v.y; p.z += P.dt * v.z;
     S.posm[i] = p;
 }

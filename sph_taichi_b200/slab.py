@@ -1,4 +1,4 @@
-"""x-slab sharding of one WCSPH, DFSPH or IISPH scene across the GPUs of a node (one process per GPU).
+"""x-slab sharding of one WCSPH, DFSPH, IISPH or PCISPH scene across the GPUs of a node (one process per GPU).
 
 The reference is single-device; this is the multi-GPU extension BASELINE.json asks for (SURVEY.md section 8e).
 
@@ -46,6 +46,14 @@ The reference is single-device; this is the multi-GPU extension BASELINE.json as
   pressure acceleration without the scatter, one more message with the first ghost layer's final pressures, the
   reactions gathered onto the owned dynamic solids, and the bodies solved on every rank from the all-gather.  Whether the sharded step beats one GPU at a given scene size depends
   on the sweep count: each sweep costs two transport groups and each batch of sweeps one host wait.
+* Sharded PCISPH: PCISPH scenes (``simulationMethod: 1``) are opt-in too: ``build_sharded(..., pcisph=True)``
+  (``run_simulation.py --gpus N --shard-pcisph``); without it they are refused (``PCISPH_SINGLE_GPU``).  They step
+  through ``sph_shard_pcisph_step``, the DFSPH step's shape with PCISPH's substep: the once-per-step ghost alignment and
+  two small exchanges per prediction-correction sweep (the predicted positions {x*, m_V}, then the new pressures) and
+  none outside the loop.  The sweep's error is the max of the ranks' partials, which is exact and independent of the
+  order, so every rank runs the same sweeps and reports bit-identical ``last_iterations`` /
+  ``last_max_density_error``.  Fluid and static solids only: dynamic solids in PCISPH are refused
+  (``DYNAMIC_SOLIDS_PCISPH``).
 * Output: ``ShardedSimulation.dump(obj_id)`` is ``ParticleSystem.dump`` of a sharded run.  It is collective: every rank
   compacts x and v of that object's owned records on the device and rank 0 receives them over the engine's own
   transport (``sph_shard_dump``), in the global cell order of the last sort.  ``run_simulation.py --gpus N`` writes
@@ -90,11 +98,17 @@ DYNAMIC_SOLIDS_WCSPH_ONLY = ("x-slab sharding of dynamic solids is WCSPH only: t
 DYNAMIC_SOLIDS_IISPH = ("x-slab sharding of dynamic solids is WCSPH only: dynamic solids in IISPH scenes are single-GPU "
                         "unless requested: build_sharded(..., iisph_bodies=True) / run_simulation.py --gpus N "
                         "--shard-iisph-bodies (sharded IISPH otherwise runs fluid and static solids)")
+PCISPH_SINGLE_GPU = ("x-slab sharding runs WCSPH (0), DFSPH (4) and IISPH (3) scenes, not simulationMethod 1 unless "
+                     "requested: x-slab sharding of a PCISPH scene is opt-in (build_sharded(..., pcisph=True), "
+                     "run_simulation.py --gpus N --shard-pcisph)")
+DYNAMIC_SOLIDS_PCISPH = ("x-slab sharding of a PCISPH scene runs fluid and static solids: dynamic solids in PCISPH "
+                         "scenes are single-GPU")
 
 
 class Solver(enum.IntEnum):
     """The solvers a scene can shard with, valued by their ``simulationMethod``."""
     WCSPH = 0
+    PCISPH = 1
     IISPH = 3
     DFSPH = 4
 
@@ -120,20 +134,26 @@ def scene_has_dynamic_solids(cfg):
     return any(o.get("isDynamic") for o in list(cfg.get_rigid_bodies() or []) + list(cfg.get_rigid_blocks() or []))
 
 
-def shard_mode(method, scene_dynamic, dynamic_solids=False, iisph=False, iisph_bodies=False):
+def shard_mode(method, scene_dynamic, dynamic_solids=False, iisph=False, iisph_bodies=False, pcisph=False):
     """The ``ShardMode`` of ``build_sharded``'s opt-ins on a scene of ``simulationMethod`` ``method`` that has dynamic
     solids or not (``scene_dynamic``); raises when that mode is not sharded.  ``iisph_bodies`` implies ``iisph`` and
-    ``dynamic_solids``."""
+    ``dynamic_solids``; ``pcisph`` shards a PCISPH scene without dynamic solids."""
     if iisph_bodies and method != 3:
         raise ValueError(f"iisph_bodies=True shards an IISPH scene (simulationMethod 3) with dynamic solids, not "
                          f"simulationMethod {method}")
+    if pcisph and method != 1:
+        raise ValueError(f"pcisph=True shards a PCISPH scene (simulationMethod 1), not simulationMethod {method}")
     if method == 3 and not (iisph or iisph_bodies):
         raise NotImplementedError(IISPH_SINGLE_GPU)
-    if method not in (0, 3, 4):
+    if method == 1 and not pcisph:
+        raise NotImplementedError(PCISPH_SINGLE_GPU)
+    if method not in (0, 1, 3, 4):
         raise NotImplementedError(f"x-slab sharding runs WCSPH (0), DFSPH (4) and IISPH (3) scenes, not "
                                   f"simulationMethod {method}")
     if iisph and method != 3:
         raise ValueError(f"iisph=True shards an IISPH scene (simulationMethod 3), not simulationMethod {method}")
+    if pcisph and (dynamic_solids or scene_dynamic):
+        raise NotImplementedError(DYNAMIC_SOLIDS_PCISPH)
     if iisph and not iisph_bodies and (dynamic_solids or scene_dynamic):
         raise NotImplementedError(DYNAMIC_SOLIDS_IISPH)
     bodies = dynamic_solids or iisph_bodies
@@ -326,7 +346,7 @@ class ShardedSimulation:
         (``dynamic_bodies``, ``startup_state``), an empty list for advected rigid blocks only; None otherwise."""
         from . import engine as _engine
         self.cfg, self.mode, self.rank, self.world, self.group = cfg, mode, rank, world, group
-        if mode.solver is not Solver.WCSPH and not n_fluid:
+        if mode.solver in (Solver.DFSPH, Solver.IISPH) and not n_fluid:
             raise ValueError("a sharded DFSPH or IISPH scene needs n_fluid, the fluid particle count of ALL ranks")
         self.device = torch.device(device)
         self.slabs0 = [tuple(int(v) for v in s_) for s_ in slabs]
@@ -340,7 +360,7 @@ class ShardedSimulation:
         self._load(mine, n_mine, uniform_hint)
         self.last_iterations_v = self.last_iterations = 0
         self._io = None
-        self.last_avg_err = 0.0
+        self.last_avg_err = self.last_max_density_error = 0.0
         # the solver is set before sph_shard_configure: the library refuses the switch on a sharded context
         if mode.solver is Solver.DFSPH:
             e.set_dfsph(True)
@@ -350,6 +370,10 @@ class ShardedSimulation:
             e.set_iisph(True)
             from .IISPH import iisph_step_io
             self._io = iisph_step_io(n_fluid)
+        elif mode.solver is Solver.PCISPH:
+            e.set_pcisph(True)
+            from .PCISPH import pcisph_step_io, scaling_factor
+            self._io = pcisph_step_io(scaling_factor(cfg.get_cfg("timeStepSize"), cfg.get_cfg("particleRadius")))
         # ---- transport: NCCL inside the library (its own communicator), or a caller-supplied one (tests) ----
         if transport is not None:
             self._transport = transport
@@ -368,7 +392,9 @@ class ShardedSimulation:
             e._check(e.lib.sph_comm_set_transport(e.ctx, None, 0, 1), "sph_comm_set_transport")
         lo, hi = self.slabs0[rank]
         args = (e.ctx, lo, hi, mode.ghost_layers, self.halo_cap, int(rebalance_every))
-        if not mode.bodies:
+        if mode.solver is Solver.PCISPH:
+            name = "sph_shard_configure_pcisph"
+        elif not mode.bodies:
             name = "sph_shard_configure"
         else:
             table = (_lib.SphRigidBody * max(1, len(self.bodies)))()
@@ -402,12 +428,17 @@ class ShardedSimulation:
     def iisph(self):
         return self.mode.solver is Solver.IISPH
 
+    @property
+    def pcisph(self):
+        return self.mode.solver is Solver.PCISPH
+
     # ---- stepping --------------------------------------------------------------------------------------
     def step(self, n=1):
         """``n`` sharded steps.  DFSPH: ``last_iterations_v`` / ``last_iterations`` (and ``last_avg_err_v`` /
         ``last_avg_err``) are those of the last step, the same on every rank; IISPH: ``last_iterations`` /
-        ``last_avg_err`` (pressure sweeps and their last average error), the same on every rank.  Both wait on the
-        device once per batch of Jacobi sweeps."""
+        ``last_avg_err`` (pressure sweeps and their last average error), the same on every rank; PCISPH:
+        ``last_iterations`` / ``last_max_density_error`` (prediction-correction sweeps and their last max density
+        error), the same bits on every rank.  All three wait on the device once per batch of sweeps."""
         e, io = self.eng, self._io
         if self.mode.solver is Solver.DFSPH:
             e._check(e.lib.sph_shard_dfsph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_dfsph_step")
@@ -416,6 +447,9 @@ class ShardedSimulation:
         elif self.mode.solver is Solver.IISPH:  # io.first_batch: in, the previous step's sweeps; out, this step's
             e._check(e.lib.sph_shard_iisph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_iisph_step")
             self.last_iterations, self.last_avg_err = int(io.iterations), float(io.avg_err)
+        elif self.mode.solver is Solver.PCISPH:
+            e._check(e.lib.sph_shard_pcisph_step(e.ctx, int(n), C.byref(io), e._stream()), "sph_shard_pcisph_step")
+            self.last_iterations, self.last_max_density_error = int(io.iterations), float(io.max_err)
         else:
             e._check(e.lib.sph_shard_step(e.ctx, int(n), e._stream()), "sph_shard_step")
         self.steps_done += int(n)
@@ -546,19 +580,20 @@ class ShardedSimulation:
 
 
 def build_sharded(scene_dict, rank, world, device, group=None, capacity_factor=1.2, rebalance_every=8, slabs=None,
-                  transport=None, dynamic_solids=False, iisph=False, iisph_bodies=False):
+                  transport=None, dynamic_solids=False, iisph=False, iisph_bodies=False, pcisph=False):
     """Assemble the scene on every rank, plan the slabs from the initial layer histogram and load this rank's
     share into a CUDA engine.  ``dynamic_solids=True`` opts in to sharding WCSPH scenes with dynamic solids
     (3 ghost layers, reactions gathered across cuts, bodies solved on every rank from an all-gather of their particles).
     ``iisph=True`` opts in to sharding an IISPH scene (fluid and static solids); ``iisph_bodies=True`` to sharding an
-    IISPH scene with dynamic solids (it implies ``iisph`` and the layout of ``dynamic_solids``).
+    IISPH scene with dynamic solids (it implies ``iisph`` and the layout of ``dynamic_solids``).  ``pcisph=True`` opts
+    in to sharding a PCISPH scene (fluid and static solids).
     Returns (ShardedSimulation, n_total)."""
     from .config_builder import SimConfig
     from .scene import assemble_particles
 
     cfg = SimConfig(scene_dict)
     mode = shard_mode(cfg.get_cfg("simulationMethod"), scene_has_dynamic_solids(cfg), dynamic_solids, iisph,
-                      iisph_bodies)
+                      iisph_bodies, pcisph)
     h, grid_num, m_V0, _ = scene_geometry(cfg)
     arrays, object_collection, _, counts = assemble_particles(cfg, 3, 2 * cfg.get_cfg("particleRadius"))
     object_ids, object_sizes = np.unique(arrays["object_id"], return_counts=True)

@@ -19,9 +19,15 @@ same position.
 across ranks in every step, and the ghost alignment; it also reports the per-step average errors of both engines.  The
 tolerance rule is test_iisph_steps_vs_oracle's: |dx| / d < 2e-3 when the sweep counts match, 5e-2 otherwise.
 
+--pcisph runs the scene with the PCISPH solver (dt = 1e-3, build_sharded(pcisph=True)) and checks the same things as
+--iisph: the prediction-correction sweep count of every step against the single engine's, counts and max density
+errors bit-identical across ranks in every step, and the ghost alignment; it also reports the per-step max errors of
+both engines.  The tolerance rule is test_pcisph_steps_vs_oracle's: |dx| / d < 1e-3 when the sweep counts match, 5e-2
+otherwise.
+
 --collide splits the fluid into two blocks (objects 0 and 1) that move toward each other at +-vx and meet at the
 initial cut of a balanced two-rank start: the fluid along the contact plane is compressed above the rest density within
-a few steps, so the pressure solves of DFSPH and IISPH run several sweeps right at the cut.
+a few steps, so the pressure solves of DFSPH, IISPH and PCISPH run several sweeps right at the cut.
 
 --dynamic-body / --dynamic-block add dynamic solids (WCSPH, build_sharded(dynamic_solids=True)): a shape-matched cube
 (tests/golden/cube.obj) straddling the fluid's x fraction 1/world (1/2 on one rank) -- the initial cut of a balanced
@@ -53,12 +59,12 @@ import torch.distributed as dist
 from sph_taichi_b200 import ParticleSystem, SimConfig, scene, slab
 
 
-def static_block_scene(c, d):
-    """The dam break one spacing above a static floor block (object 1, three lattice layers thick) that spans twice
+def static_block_scene(c, d, gap=1.0):
+    """The dam break ``gap`` spacings above a static floor block (object 1, three lattice layers thick) that spans twice
     the fluid's x extent and its whole z extent: every cut of the fluid also cuts the block, and the fluid slides
     along it."""
     sc = scene.dam_break_box(c, domain_end=[2.5 * c[0] * d + 0.2, c[1] * d + 0.4, c[2] * d + 0.12],
-                             start=[0.06, 0.10, 0.06])
+                             start=[0.06, 0.10 + (gap - 1.0) * d, 0.06])
     lo = [0.04, 0.04, 0.04]
     n = [2 * c[0], 3, c[2] + 2]
     sc["RigidBlocks"] = [{"objectId": 1, "start": lo, "end": [s + (k - 0.5) * d for s, k in zip(lo, n)],
@@ -121,8 +127,13 @@ def main():
     ap.add_argument("--dfsph", action="store_true", help="DFSPH instead of WCSPH (simulationMethod 4, dt = 4e-3)")
     ap.add_argument("--iisph", action="store_true",
                     help="IISPH instead of WCSPH (simulationMethod 3, dt = 1e-3; build_sharded(iisph=True))")
+    ap.add_argument("--pcisph", action="store_true",
+                    help="PCISPH instead of WCSPH (simulationMethod 1, dt = 1e-3; build_sharded(pcisph=True))")
     ap.add_argument("--static-block", action="store_true",
                     help="the fluid rests on a static rigid block that straddles every cut (static_block_scene)")
+    ap.add_argument("--block-gap", type=float, default=1.0,
+                    help="with --static-block: lattice spacings between the block's top layer and the fluid's bottom "
+                         "layer")
     ap.add_argument("--collide", action="store_true",
                     help="two fluid blocks meeting at +-vx at the initial cut (colliding_blocks_scene)")
     ap.add_argument("--dynamic-body", action="store_true",
@@ -132,7 +143,8 @@ def main():
     ap.add_argument("--body-vy", type=float, default=0.0, help="initial vertical velocity of the dynamic solids")
     ap.add_argument("--scene", default=None, choices=sorted(scene.NAMED_SCENES),
                     help="a named scene as it is (--counts, --vx and --static-block do not apply; a DFSPH scene needs "
-                         "--dfsph for the iteration-count comparison, an IISPH scene --iisph)")
+                         "--dfsph for the iteration-count comparison, an IISPH scene --iisph, a PCISPH scene "
+                         "--pcisph)")
     ap.add_argument("--soak", type=int, default=0, metavar="EVERY",
                     help="long run: read the step state (capacity / out-of-grid flags raise) every EVERY steps; the "
                          "flow is chaotic over thousands of steps, so the verdict is the particle set, finiteness and "
@@ -153,7 +165,7 @@ def main():
         sc = scene.NAMED_SCENES[a.scene]()
         d = 2.0 * sc["Configuration"]["particleRadius"]
     elif a.static_block:
-        sc = static_block_scene(c, d)
+        sc = static_block_scene(c, d, a.block_gap)
     elif a.collide:
         sc = colliding_blocks_scene(c, d, a.vx)
     else:
@@ -169,7 +181,9 @@ def main():
         sc = scene._as_dfsph(sc)
     if a.iisph and sc["Configuration"]["simulationMethod"] != 3:
         sc = scene._as_iisph(sc)
-    jacobi = a.dfsph or a.iisph  # one step per call, sweep counts and the ghost alignment checked
+    if a.pcisph and sc["Configuration"]["simulationMethod"] != 1:
+        sc = scene._as_pcisph(sc)
+    jacobi = a.dfsph or a.iisph or a.pcisph  # one step per call, sweep counts and the ghost alignment checked
     transport = slab.GlooTransport() if (EMU and world > 1) else None
     slabs = None
     if a.skew:  # deliberately unbalanced start: every interior cut shifted, the balancer has to move them back
@@ -184,7 +198,7 @@ def main():
         slabs = [(cuts[r], cuts[r + 1]) for r in range(world)]
     sim, n_total = slab.build_sharded(sc, rank, world, dev, rebalance_every=a.rebalance_every, slabs=slabs,
                                       transport=transport, dynamic_solids=dynamic, iisph=a.iisph,
-                                      iisph_bodies=bool(a.iisph and dynamic))
+                                      iisph_bodies=bool(a.iisph and dynamic), pcisph=a.pcisph)
     first = sim.info()
     trace = []
 
@@ -208,6 +222,10 @@ def main():
         for _ in range(a.steps):  # one step per call: the sweep counts of every step
             sim.step(1)
             trace.append((sim.last_iterations, sim.last_avg_err.hex()) + ((body_trace(),) if sim.mode.bodies else ()))
+    elif a.pcisph:
+        for _ in range(a.steps):  # one step per call: the sweep counts and max errors of every step
+            sim.step(1)
+            trace.append((sim.last_iterations, sim.last_max_density_error.hex()))
     elif sim.mode.bodies:
         for _ in range(a.steps):  # one step per call: the body states of every step
             sim.step(1)
@@ -249,6 +267,11 @@ def main():
                 s.step(1)
                 single_counts.append([s.last_iterations])
                 single_errs.append(float(s.last_avg_density_error))
+        elif a.pcisph:
+            for _ in range(a.steps):
+                s.step(1)
+                single_counts.append([s.last_iterations])
+                single_errs.append(float(s.last_max_density_error))
         else:
             s.step(a.steps)
         bodies = None
@@ -279,9 +302,9 @@ def main():
                 aligned = aligned and gl == metas[r - 1]["x0_owned"][len(metas[r - 1]["x0_owned"]) - len(gl):]
                 aligned = aligned and gr == metas[r]["x0_owned"][:len(gr)]
             counts_match = counts == single_counts
-            # the rule of test_dfsph_steps_vs_oracle / test_iisph_steps_vs_oracle: tight when the solvers ran the same
-            # sweeps
-            tol = 2e-3 if counts_match else 5e-2
+            # the rule of test_dfsph_steps_vs_oracle / test_iisph_steps_vs_oracle / test_pcisph_steps_vs_oracle: tight
+            # when the solvers ran the same sweeps
+            tol = (1e-3 if a.pcisph else 2e-3) if counts_match else 5e-2
             ok = (cmp_["same_particle_set"] and cmp_["max_dx_over_d"] < tol and same_on_ranks and aligned
                   and slab.static_solids_ok(cmp_))
             cmp_ = dict(cmp_, iterations_sharded=counts, iterations_single=single_counts, counts_match=counts_match,
@@ -290,6 +313,8 @@ def main():
                         transport_bytes=[m["transport"][1] for m in metas])
             if a.iisph:
                 cmp_.update(avg_err_sharded=[float.fromhex(t[1]) for t in metas[0]["trace"]], avg_err_single=single_errs)
+            if a.pcisph:
+                cmp_.update(max_err_sharded=[float.fromhex(t[1]) for t in metas[0]["trace"]], max_err_single=single_errs)
         if sim.mode.bodies:
             same_on_ranks = all(json.dumps(m["trace"]) == json.dumps(metas[0]["trace"]) for m in metas)
             g_y, t = float(sc["Configuration"]["gravitation"][1]), a.steps * float(sc["Configuration"]["timeStepSize"])

@@ -1,4 +1,5 @@
-"""Sharded IISPH at world 1 against the plain IISPH engine, on one GPU, in one process.
+"""Sharded IISPH (or PCISPH, `--pcisph`) at world 1 against the plain engine of the same solver, on one GPU, in one
+process.
 
 Both engines run `--scene` (default dragon_bath_iisph) from the same start.  After `--warmup` steps each, the timed
 window is `--rounds` rounds of `--steps` steps, alternating plain and sharded, so that both are timed on states at the
@@ -13,7 +14,11 @@ profiles/h100_shard_iisph_timing.json) and prints a summary line.
 also rebuilds the solid-id slot map, computes the moving boundary volumes through it, gathers the reactions instead of
 scattering them and solves the bodies from the packed table of their particles.
 
-    python tools/shard_iisph_timing.py [--bodies] [--steps 20] [--rounds 5] [--warmup 30] [--out PATH]
+`--pcisph` times sharded PCISPH instead (scene dragon_bath_pcisph, built with `build_sharded(pcisph=True)`; default
+output profiles/h100_shard_pcisph_timing.json): the sweeps are prediction-correction sweeps, and the sharded loop
+check takes the max of the ranks' error partials.
+
+    python tools/shard_iisph_timing.py [--bodies | --pcisph] [--steps 20] [--rounds 5] [--warmup 30] [--out PATH]
 """
 import argparse
 import json
@@ -44,22 +49,26 @@ def timed(step, last_sweeps, k):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scene", default=None, help="default: dragon_bath_iisph, with --bodies "
-                                                  "armadillo_bath_dynamic_iisph")
-    ap.add_argument("--bodies", action="store_true", help="a scene with dynamic solids: build_sharded(iisph_bodies=True)")
+                                                  "armadillo_bath_dynamic_iisph, with --pcisph dragon_bath_pcisph")
+    mode = ap.add_mutually_exclusive_group()
+    mode.add_argument("--bodies", action="store_true", help="a scene with dynamic solids: build_sharded(iisph_bodies=True)")
+    mode.add_argument("--pcisph", action="store_true", help="a PCISPH scene: build_sharded(pcisph=True)")
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=30)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    a.scene = a.scene or ("armadillo_bath_dynamic_iisph" if a.bodies else "dragon_bath_iisph")
-    a.out = a.out or os.path.join(ROOT, "profiles", "h100_shard_iisph_bodies_timing.json" if a.bodies
-                                  else "h100_shard_iisph_timing.json")
+    kind = "pcisph" if a.pcisph else "iisph_bodies" if a.bodies else "iisph"
+    a.scene = a.scene or {"pcisph": "dragon_bath_pcisph", "iisph_bodies": "armadillo_bath_dynamic_iisph",
+                          "iisph": "dragon_bath_iisph"}[kind]
+    a.out = a.out or os.path.join(ROOT, "profiles", f"h100_shard_{kind}_timing.json")
     dev = torch.device("cuda:0")
     sc = scene.NAMED_SCENES[a.scene]()
     ps = ParticleSystem(SimConfig(sc), device=dev)
     solver = ps.build_solver()
     solver.initialize()
-    sim, n_total = slab.build_sharded(scene.NAMED_SCENES[a.scene](), 0, 1, dev, iisph=True, iisph_bodies=a.bodies)
+    opt_in = {"pcisph": True} if a.pcisph else {"iisph": True, "iisph_bodies": a.bodies}
+    sim, n_total = slab.build_sharded(scene.NAMED_SCENES[a.scene](), 0, 1, dev, **opt_in)
     engines = {"plain": (lambda: solver.step(1), lambda: int(solver.last_iterations)),
                "sharded_world1": (lambda: sim.step(1), lambda: int(sim.last_iterations))}
     for step, _ in engines.values():
